@@ -1,4 +1,4 @@
-"""auto_round_b200 -- B200-native (sm_100a) engine for the AutoRound block-wise SignRound calibration path.
+"""auto_round_b200 -- H100-native (sm_90a) engine for the AutoRound block-wise SignRound calibration path.
 
 Public surface mirrors the reference for this path only: `AutoRound(...).quantize()/quantize_and_save()`,
 `QuantizationScheme` presets, the `auto_round` checkpoint format.  Compute is hand-written CUDA behind the C ABI

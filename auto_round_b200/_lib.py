@@ -79,7 +79,7 @@ def load() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise RuntimeError(f"{LIB_PATH} not found: run `python -m auto_round_b200.build` (nvcc, sm_100a). "
+        raise RuntimeError(f"{LIB_PATH} not found: run `python -m auto_round_b200.build` (nvcc, sm_90a). "
                            "auto_round_b200 has no CPU or eager-PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     lib.ar_version.restype = C.c_int

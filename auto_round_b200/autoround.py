@@ -1,6 +1,6 @@
 """`AutoRound(...)` entry point -- keeps the reference's Python surface for the block-wise tuning path
 (auto_round/autoround.py:722-788; compressors/base.py:202-486, :1925-2021; compressors/orchestrator.py:176-388,
-:525-816; algorithms/composer.py:360-483) while every kernel of the hot path is hand-written sm_100a CUDA.
+:525-816; algorithms/composer.py:360-483) while every kernel of the hot path is hand-written sm_90a CUDA.
 
     ar = AutoRound(model, tokenizer, scheme="W4A16", iters=200, nsamples=128, seqlen=2048, batch_size=8,
                    dataset=[LongTensor[b, seqlen], ...], device_map=0, seed=42)
@@ -61,7 +61,7 @@ def find_blocks(model: nn.Module):
 
 
 class _GemmLinear(nn.Module):
-    """nn.Linear forward on the tcgen05 GEMM (used for the no-grad full-set block forwards)."""
+    """nn.Linear forward on the wgmma GEMM (used for the no-grad full-set block forwards)."""
 
     def __init__(self, lin: nn.Linear):
         super().__init__()
@@ -172,15 +172,15 @@ class AutoRound:
         if platform != "hf":
             raise NotImplementedError("only platform='hf'")
         if algorithm not in (None, "signround") or alg_configs is not None:
-            raise NotImplementedError("only the default SignRound algorithm is built on B200")
+            raise NotImplementedError("only the default SignRound algorithm is built on H100")
         if enable_torch_compile:
-            raise NotImplementedError("torch.compile is not part of the B200 path (hand-written kernels instead)")
+            raise NotImplementedError("torch.compile is not part of the H100 path (hand-written kernels instead)")
         unknown = set(kwargs) - set(_SCHEME_KW) - set(_SIGNROUND_KW)
         if unknown:
-            raise TypeError(f"unsupported AutoRound arguments for the B200 hot path: {sorted(unknown)}")
+            raise TypeError(f"unsupported AutoRound arguments for the H100 hot path: {sorted(unknown)}")
         for k in ("enable_norm_bias_tuning", "enable_lfq"):
             if kwargs.get(k):
-                raise NotImplementedError(f"{k}=True is outside the B200 hot path")
+                raise NotImplementedError(f"{k}=True is outside the H100 hot path")
         # quant_lm_head: SURVEY.md 8 f4 (quantize_layer_outside_block).  Oracle pinned against a reference run
         # (tests/golden/lm_head_*.pt); CUDA loop: quantizer.quantize_layer, GPU parity in tests/test_gpu_lm_head.py
         self.quant_lm_head = bool(kwargs.get("quant_lm_head"))
@@ -245,7 +245,7 @@ class AutoRound:
         else:
             raise TypeError(f"device_map {device_map!r} not supported (one GPU per process; use torchrun for DP)")
         if dev.type != "cuda":
-            raise RuntimeError("auto_round_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("auto_round_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         return dev
 
     @staticmethod

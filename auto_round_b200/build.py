@@ -1,9 +1,9 @@
-"""Build libar_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libar_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
     python -m auto_round_b200.build [--force]
 
-nvcc cross-compiles for sm_100a without a GPU.  The .so is git-ignored but travels to the GPU box with the
-repo snapshot.  `-fmad=false`: the fake-quant numerics must not be contracted into FMAs (bit-exact parity
+nvcc cross-compiles for sm_90a (H100) without a GPU.  The objects and the .so are build products (git-ignored);
+they are rebuilt when a source, a header or this file (the flags) is newer.  `-fmad=false`: the fake-quant numerics must not be contracted into FMAs (bit-exact parity
 with the reference's separate mul/add/div ops, see csrc/ar_qdq_math.cuh).
 """
 from __future__ import annotations
@@ -17,7 +17,7 @@ CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libar_b200.so")
 SOURCES = ["ar_capi.cu", "ar_qdq.cu", "ar_pack.cu", "ar_loop.cu", "ar_block.cu", "ar_search.cu", "ar_outlier.cu", "ar_moe.cu", "ar_gemm.cu"]
 HEADERS = ["ar_common.cuh", "ar_qdq_math.cuh", os.path.join("..", "..", "include", "ar_b200.h")]
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-fmad=false",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 
 
@@ -36,7 +36,8 @@ def _stale(target: str, deps: list[str]) -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    hdrs = [os.path.join(CSRC, h) for h in HEADERS]
+    # the flags live in this file: editing it rebuilds everything
+    hdrs = [os.path.join(CSRC, h) for h in HEADERS] + [os.path.abspath(__file__)]
     objs, jobs = [], []
     for src in SOURCES:
         s = os.path.join(CSRC, src)
@@ -56,7 +57,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
             list(ex.map(run, jobs))
     if jobs or force or _stale(LIB, objs):
-        run([_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"])
+        run([_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"])
     return LIB
 
 

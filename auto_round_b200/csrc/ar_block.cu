@@ -1,7 +1,6 @@
 // Fused elementwise ops of a Llama-family decoder block (the glue between the fake-quant linears inside the
 // sign-SGD iteration): RMSNorm, rotary embedding, SwiGLU -- forward and backward, one HBM pass each.
-// They replace ~40 ATen elementwise launches per iteration (profiles/r01_launches_bench.md: 28 % of the
-// iteration's device time) with 10.  Forward values reproduce the HF eager op order bit-for-bit
+// They replace ~40 ATen elementwise launches per iteration with 10.  Forward values reproduce the HF eager op order bit-for-bit
 // (fp32 math, bf16 rounding at the same points):
 //   LlamaRMSNorm.forward      transformers/models/llama/modeling_llama.py  (x.float() -> *rsqrt(mean(x^2)+eps) -> bf16 -> *w)
 //   apply_rotary_pos_emb      (q*cos) + (rotate_half(q)*sin), each product and the sum rounded to bf16

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libar_b200.so.
+// Shared helpers for the sm_90a kernels of libar_b200.so.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -3,7 +3,7 @@
 // nonzero / index_select / index_copy_ per expert) with
 //
 //   ar_moe_route     top-k expert ids [T, k]  ->  a layout of the (token, slot) pairs SORTED BY EXPERT, every expert's segment
-//                    padded to the 256-row GEMM tile, plus the tile tables the grouped tcgen05 GEMMs walk
+//                    padded to the 256-row GEMM tile, plus the tile tables the grouped wgmma GEMMs walk
 //   ar_moe_gather    Xp[row] = X[token(row)] (optionally * the routing weight of that pair), pad rows = 0
 //   ar_moe_combine   out[token] = sum over its k slots of (D[row(token, slot)] * w[token, slot])   (gather form: deterministic,
 //                    no atomics -- the reference's `.view(ntok, k, -1).sum(dim=1)`)

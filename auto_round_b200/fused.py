@@ -2,7 +2,7 @@
 block for the duration of the tuning loop and of the full-set forwards.
 
 The reference runs these as chains of ATen elementwise kernels inside the HF layer (the layer is user code from
-`transformers`, reached through compressors/utils.py:109-172 block_forward).  On B200 they are ~28 % of an iteration's
+`transformers`, reached through compressors/utils.py:109-172 block_forward).  They are a visible share of an iteration's
 device time, so each chain becomes one hand-written kernel forward and one backward (csrc/ar_block.cu).  Forward
 values keep HF's rounding points; blocks that do not match the recognised patterns are left untouched.
 """

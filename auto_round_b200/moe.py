@@ -1,6 +1,6 @@
-"""MoE experts on B200 -- replaces auto_round/modeling/fused_moe/moe_experts_interface.py:173-260 (the reference un-fuses
+"""MoE experts on H100 -- replaces auto_round/modeling/fused_moe/moe_experts_interface.py:173-260 (the reference un-fuses
 HF's fused 3-D expert parameters into per-expert nn.Linear modules and runs a python loop over the experts with
-nonzero / index_select / index_copy_ per expert) by a device-side routing + grouped tcgen05 GEMM path:
+nonzero / index_select / index_copy_ per expert) by a device-side routing + grouped wgmma GEMM path:
 
     ar_moe_route      (token, slot) pairs sorted by expert, segments padded to the 256-row tile, tile tables   csrc/ar_moe.cu
     ar_moe_gather     Xp = X[token of row]                                                                       "

@@ -1,5 +1,5 @@
 """Thin torch-tensor front end over the C ABI (include/ar_b200.h).  PyTorch only owns the memory and the
-stream; every function below enqueues hand-written sm_100a kernels from libar_b200.so and returns.
+stream; every function below enqueues hand-written sm_90a kernels from libar_b200.so and returns.
 
 No function here has a CPU / eager fallback: tensors must be CUDA tensors and the library must load.
 """
@@ -62,7 +62,7 @@ def make_spec(name: str, bits: int, group_size: int, n: int, k: int, q_scale_thr
     """group_size -1, or a weight narrower than the group (K < group_size), means one group per ROW in the reference
     (reshape_pad_tensor_by_group_size, data_type/utils.py:57-61): encoded as group_size == K (int types only)."""
     if group_size == 0:
-        raise NotImplementedError("group_size = 0 (one group per tensor) is outside the B200 hot path")
+        raise NotImplementedError("group_size = 0 (one group per tensor) is outside the H100 hot path")
     if group_size == -1 or k < group_size:
         if name not in ("int_sym", "int_asym"):
             raise NotImplementedError(f"{name}: per-row groups (group_size=-1 / K < group_size) exist for the int types only")
@@ -163,7 +163,7 @@ def qdq_bwd(spec: Spec, w, gq, v=None, min_scale=None, max_scale=None, wmin=None
 
 
 def gemm(a, b, a_mn_major=False, b_mn_major=False, bias=None, out=None):
-    """D[M,N] = A·Bᵀ on tcgen05.  A is [M,K] (or stored [K,M] if a_mn_major), B is [N,K] (or stored [K,N])."""
+    """D[M,N] = A·Bᵀ on wgmma.  A is [M,K] (or stored [K,M] if a_mn_major), B is [N,K] (or stored [K,N])."""
     _want(a, torch.bfloat16, "a")
     _want(b, torch.bfloat16, "b")
     if a_mn_major:

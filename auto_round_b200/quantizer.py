@@ -1,13 +1,13 @@
-"""Block-wise SignRound tuning on B200 -- host-side mirror of
+"""Block-wise SignRound tuning on H100 -- host-side mirror of
 auto_round/algorithms/quantization/sign_round/quantizer.py:311-552 (SignRoundQuantizer.quantize_block).
 
 Same call contract as the reference's plug point (SURVEY.md 8b #1): `quantize_block(block, fp_inputs, input_others,
 fp_outputs, q_inputs, block_ctx, input_ids=None)` mutates `block` in place (qdq weights, `.scale/.zp/
 .weight_global_scale` attributes on every quantised nn.Linear) and returns the best parameters.
 
-What is different from the reference (B200-first):
+What is different from the reference (H100-first):
   * all tunables of a block live in ONE flat fp32 arena [V of every layer | scales of every layer] with a matching
-    best-snapshot arena; the weight gradient of every layer is the bf16 dWq of a plain tcgen05 GEMM, and ONE fused kernel
+    best-snapshot arena; the weight gradient of every layer is the bf16 dWq of a plain wgmma GEMM, and ONE fused kernel
     per layer turns it into (fake-quant backward -> snapshot -> sign-SGD step -> next iteration's fake-quant weight);
   * under data parallelism a layer's dWq is reduce-scattered over the ranks as soon as its backward GEMMs are issued
     (overlapping the rest of the backward), each rank updates its row shard of V / scales and the new fake-quant weight

@@ -40,7 +40,7 @@ class QuantizationScheme:
             return "mx_fp4"
         if dt in ("nv_fp", "nv_fp4") and self.bits == 4:
             return "nv_fp4"
-        raise NotImplementedError(f"data_type={dt!r} bits={self.bits} is outside the B200 hot path "
+        raise NotImplementedError(f"data_type={dt!r} bits={self.bits} is outside the H100 hot path "
                                   "(int 2/3/4/8, mx_fp4, nv_fp4)")
 
     @property
@@ -85,7 +85,7 @@ def parse_scheme(scheme, overrides: Optional[dict] = None) -> QuantizationScheme
         s.act_bits = 16
     if not s.weight_only:
         raise NotImplementedError(
-            "activation quantisation (act_bits < 16) is outside the B200 hot path; pass act_bits=16 "
+            "activation quantisation (act_bits < 16) is outside the H100 hot path; pass act_bits=16 "
             "(and act_data_type='float' for NVFP4) for weight-only tuning, as BASELINE.json's configs do")
     s.qdq_name  # validates the weight data type
     return s

@@ -2,9 +2,9 @@
 
 `WrapperLinear` keeps the reference's parameter names (`value`, `min_scale`, `max_scale`, wrapper.py:184-190)
 but the parameters are *views into one flat fp32 arena per block* (see quantizer.TuneArena) and the math runs in
-hand-written sm_100a kernels behind the C ABI:
+hand-written sm_90a kernels behind the C ABI:
 
-    forward   ar_gemm_bf16          Y = X · Wqᵀ on tcgen05; Wq = qdq(W; V, scales) is resident     (wrapper.py:517-565)
+    forward   ar_gemm_bf16          Y = X · Wqᵀ on wgmma;  Wq = qdq(W; V, scales) is resident     (wrapper.py:517-565)
     backward  ar_gemm_bf16          dWq = dYᵀ·X  (bf16, like autograd of F.linear)  and  dX = dY · Wq
               ar_fq_update          ONE pass per layer: fake-quant backward from dWq (replaces autograd through
                                     wrapper.py:273-290), best-param snapshot, sign-SGD step, and the NEXT iteration's Wq

@@ -1,7 +1,8 @@
-"""bench.py -- block-wise SignRound calibration on B200; headline: Llama-3-8B W4A16 (sym, g128), BASELINE.json configs[1].
+"""bench.py -- block-wise SignRound calibration on H100; headline: Llama-3-8B W4A16 (sym, g128), BASELINE.json configs[1].
 
     python bench.py --gpus N --steps K --warmup W [--config NAME]      # our arm  (torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K --warmup W     # the reference's CPU path (oracle port)
+    python bench.py ... --dump-outputs DIR                              # + the last timed block's packed tensors as .npy
 
 A STEP is one transformer block taken through the whole hot path exactly as the reference's `quantization tuning time`
 span counts it (compressors/orchestrator.py:631 -> 792): FP reference forward over all 128 calibration samples, `iters`
@@ -50,15 +51,15 @@ CONFIGS = {
     "llama3_8b_w4a16": dict(
         metric="Llama-3-8B W4A16 calib wall-clock (s) @200 iters", model="llama3_8b", n_blocks=32, iters=200,
         scheme=dict(scheme="W4A16"), spec=("int_sym", 4, 128), linears=_LLAMA_LIN,
-        workload="Llama-3-8B W4A16 sym g128 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxB200"),
+        workload="Llama-3-8B W4A16 sym g128 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxH100"),
     "w2asym_algext": dict(
         metric="Llama-3-8B W2A16 asym g32 enable_alg_ext calib wall-clock (s) @1000 iters", model="llama3_8b", n_blocks=32,
         iters=1000, scheme=dict(scheme="W2A16", group_size=32, sym=False, enable_alg_ext=True), spec=("int_asym", 2, 32),
-        linears=_LLAMA_LIN, workload="Llama-3-8B W2A16 asym g32 enable_alg_ext iters=%d nsamples=128 seqlen=2048 batch=8 on %dxB200"),
+        linears=_LLAMA_LIN, workload="Llama-3-8B W2A16 asym g32 enable_alg_ext iters=%d nsamples=128 seqlen=2048 batch=8 on %dxH100"),
     "qwen2_nvfp4": dict(
         metric="Qwen2-7B NVFP4 (weight-only) calib wall-clock (s) @200 iters", model="qwen2_7b", n_blocks=28, iters=200,
         scheme=dict(scheme="NVFP4", act_bits=16, act_data_type="float"), spec=("nv_fp4", 4, 16), linears=_QWEN_LIN,
-        workload="Qwen2-7B NVFP4 weight-only g16 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxB200"),
+        workload="Qwen2-7B NVFP4 weight-only g16 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxH100"),
 }
 _MIXTRAL_LIN = [("q", 4096, 4096, False), ("k", 1024, 4096, False), ("v", 1024, 4096, False), ("o", 4096, 4096, True),
                 # top-2 of 8 experts: per token two gate / up / down projections are active (the FLOP count of a step)
@@ -68,7 +69,7 @@ CONFIGS["mixtral_mxfp4"] = dict(
     metric="Mixtral-8x7B MXFP4 (weight-only) calib wall-clock (s) @200 iters", model="mixtral_8x7b", n_blocks=32, iters=200,
     scheme=dict(scheme="MXFP4", act_bits=16), spec=("mx_fp4", 4, 32), linears=_MIXTRAL_LIN,
     p_block=4096 * 4096 * 2 + 1024 * 4096 * 2 + 8 * 3 * 14336 * 4096,
-    workload="Mixtral-8x7B MXFP4 weight-only g32 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxB200")
+    workload="Mixtral-8x7B MXFP4 weight-only g32 iters=%d nsamples=128 seqlen=2048 batch=8 on %dxH100")
 MODELS = {
     "mixtral_8x7b": ("MixtralConfig", "MixtralForCausalLM", dict(hidden_size=4096, intermediate_size=14336, num_attention_heads=32,
                                                               num_key_value_heads=8, vocab_size=32000, rope_theta=1000000.0,
@@ -93,13 +94,13 @@ def flops_per_step(cfg, iters):
 
 def peaks():
     """MEASURED_PEAKS.json (driver-written): `bf16_tflops` = burst (a kernel timed alone), `bf16_tflops_sustained` = inside
-    a long step; fallback = B200_PROFILING.md."""
+    a long step; fallback = NVIDIA's H100 SXM data sheet (dense bf16 / HBM3 at 700 W), a ceiling rather than a measured rate."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"burst": d.get("bf16_tflops"), "sustained": d.get("bf16_tflops_sustained", d.get("bf16_tflops")),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "MEASURED_PEAKS.json"}
-    return {"burst": 1650.0, "sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"burst": 989.0, "sustained": 989.0, "hbm_gbs": 3350.0, "source": "fallback (H100 SXM data sheet, 700 W)"}
 
 
 class ClockSampler(threading.Thread):
@@ -210,7 +211,7 @@ def line_config(cfg, iters, world, n_measured):
             "parallelism": "dp%d (calibration samples sharded; per layer: reduce-scatter of the bf16 dWq, row-sharded fused update, "
                            "all-gather of the next fake-quant weight, overlapped with the backward%s)"
                            % (world, "; MoE experts: expert-parallel ownership, all-gather of tokens + reduce-scatter of outputs" if "mixtral" in cfg["model"] else ""),
-            "l2": "inputs larger than L2 (per-iteration working set 3.4 GB >> 126 MB)"}
+            "l2": "inputs larger than L2 (per-iteration working set 3.4 GB >> 50 MB)"}
 
 
 def run_ours(args):
@@ -340,9 +341,39 @@ def run_ours(args):
             line["cpu_baseline"] = cpu_baseline(cfg, steps=8, warmup=1, budget_s=args.cpu_budget)
     else:
         line["roofline"] = {"bound": "tensor", "note": "measured at N=1 (same kernels); see the N=1 line"}
+    if args.dump_outputs:
+        line["dumped_outputs"] = {"block": W + K - 1, **dump_outputs(model.model.layers[W + K - 1], args.dump_outputs)}
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_BUDGET_BYTES = 60 << 20          # below 64 MB with the .npy headers
+
+
+def dump_outputs(block, out_dir):
+    """The packed tensors of the last timed block (what `quantize()` hands the caller for it: qweight / qzeros / scales /
+    g_idx of every quantized linear) as DIR/<layer>.<buffer>.npy -- integers as float64 (exact), floats as float32.  A
+    tensor larger than its share of the budget is replaced by a fixed sample (seed 0, sorted flat indices), so two builds
+    run with the same arguments can be compared element for element."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    bufs = [(n, b) for n, b in block.named_buffers() if b.numel() > 0]
+    share = DUMP_BUDGET_BYTES // max(len(bufs), 1)
+    written = {}
+    for name, b in bufs:
+        flat = b.detach().cpu().reshape(-1)
+        as64 = not flat.is_floating_point()
+        cap = share // (8 if as64 else 4)
+        sampled = flat.numel() > cap
+        if sampled:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+            flat = flat[idx]
+        arr = flat.to(torch.float64 if as64 else torch.float32).numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), arr if sampled else arr.reshape(tuple(b.shape)))
+        written[name] = {"shape": list(b.shape), "sampled": cap if sampled else None}
+    return {"dir": out_dir, "tensors": written}
 
 
 def collective_probe(dev, world, cfg):
@@ -424,15 +455,10 @@ def gemm_roofline(dev, pk, cfg):
     torch.cuda.synchronize()
     ms = s.elapsed_time(e) / reps
     achieved = flops / (ms / 1e3) / 1e12
-    traffic, tsrc = None, None
-    tp = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if os.path.exists(tp):
-        td = json.load(open(tp))
-        traffic, tsrc = td.get("dram_bytes_per_launch_avg"), td.get("source")
-    return {"bound": "tensor", "kernel": "ar::gemm_kernel (tcgen05 cta_group::2, 256x256x64 tiles, dynamic tile scheduler; fwd / grad-in / grad-w)",
+    return {"bound": "tensor", "kernel": "ar::gemm_kernel (wgmma, 128x128x64 tiles, dynamic tile scheduler; fwd / grad-in / grad-w)",
             "achieved": round(achieved, 1), "peak": pk["burst"], "unit": "TFLOP/s", "frac": round(achieved / pk["burst"], 4),
             "peak_source": pk["source"] + " bf16_tflops (burst: the replay is an isolated ~0.2 s run)",
-            "traffic": traffic, "traffic_source": tsrc, "flops_per_launch": flops // nlaunch,
+            "flops_per_launch": flops // nlaunch,
             "algorithmic_bytes_per_launch": int(sum(2 * (BATCH * SEQLEN * (n + k) + n * k) * (3 if dx else 2)
                                                     for _, n, k, dx in cfg["linears"]) / nlaunch),
             "avg_launch_ms": round(ms / nlaunch, 4), "launches_per_iteration": nlaunch,
@@ -587,7 +613,7 @@ def mse_vs_reference(ar, model, orig_block0, cfg, iters, dev, line):
     steady = sorted(times[3:])
     eager_ms = 1e3 * steady[len(steady) // 2]
     line["gpu_eager_baseline"] = {
-        "what": "the reference's algorithm as torch eager + autograd on the same B200 (oracle/signround.py on cuda: ATen fake-quant "
+        "what": "the reference's algorithm as torch eager + autograd on the same GPU (oracle/signround.py on cuda: ATen fake-quant "
                 "graph, cuBLAS GEMMs, SDPA) -- the reference's GPU path without torch.compile",
         "ms_per_iteration": round(eager_ms, 2), "ours_ms_per_iteration": line["ms_per_iteration"],
         "speedup_per_iteration": round(eager_ms / line["ms_per_iteration"], 2),
@@ -740,6 +766,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-mse-check", action="store_true")
     ap.add_argument("--cpu-budget", type=float, default=60.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed block's packed tensors as DIR/<name>.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * ar_b200.h -- C ABI of the B200-native AutoRound calibration kernels (libar_b200.so).
+ * ar_b200.h -- C ABI of the H100-native AutoRound calibration kernels (libar_b200.so).
  *
  * Drop-in boundary for ONE hot path of intel/auto-round: the per-block SignRound tuning loop, its
  * weight quant-dequant numerics and the final low-bit pack.  The reference has no native code on this
@@ -43,7 +43,7 @@ enum {
   AR_OK = 0,
   AR_E_BADARG = -1,     /* null pointer / shape not supported */
   AR_E_UNSUPPORTED = -2,/* combination not built (e.g. group size) */
-  AR_E_NOTSM100 = -3,   /* tcgen05 path requested on a non-sm_100 device */
+  AR_E_ARCH = -3,       /* wgmma path requested on a device that is not sm_90 */
   AR_E_DRIVER = -4      /* cuTensorMapEncodeTiled unavailable / failed */
 };
 
@@ -106,7 +106,7 @@ int ar_qdq_mx_fp4_fwd(const ar_qspec*, const void*, const float*, const float*, 
 int ar_qdq_nv_fp4_fwd(const ar_qspec*, const void*, const float*, const float*, const float*, void*, void*, void*);
 
 /*
- * bf16 GEMM on tcgen05/TMA:  D[M,N] = A · Bᵀ  with A logical [M,K], B logical [N,K].
+ * bf16 GEMM on wgmma/TMA:  D[M,N] = A · Bᵀ  with A logical [M,K], B logical [N,K].
  *   a_mn_major / b_mn_major = 0: operand stored [rows, K] row-major (K contiguous);
  *                            = 1: operand stored [K, rows] row-major (rows contiguous).
  *   lda/ldb/ldd: leading dimension (elements) of the stored matrix.  D is bf16 row-major [M,N].
@@ -117,7 +117,7 @@ int ar_gemm_bf16(const void* a, const void* b, void* d, int m, int n, int k, int
                  int64_t lda, int64_t ldb, int64_t ldd, const void* bias_bf16, void* stream);
 
 /*
- * Grouped (ragged per-expert) bf16 GEMM on tcgen05 for un-fused MoE experts -- replaces the per-expert python loop of
+ * Grouped (ragged per-expert) bf16 GEMM on wgmma for un-fused MoE experts -- replaces the per-expert python loop of
  * auto_round/modeling/fused_moe/moe_experts_interface.py:173-260 (`_run_experts_with_routes`).  Tiles are resolved through the
  * device-side tables written by ar_moe_route in the same stream, so the launch is static (CUDA-graph capturable):
  *   mode 1 (GROUP_M)  D[rows, n] = A[rows, k] · B_eᵀ,  e = expert of each 256-row tile (table: {m0, expert} x *num).
@@ -168,8 +168,8 @@ int ar_fq_linear_fwd(const ar_qspec* q, const void* x_bf16, int64_t t, const voi
 int ar_fq_linear_bwd_dx(const ar_qspec* q, const void* dy_bf16, int64_t t, const void* wq_bf16, void* dx_bf16,
                         void* stream);
 /*
- * dWq[N,K] = dYᵀ·X on tcgen05 with the qdq backward fused in the epilogue: the fp32 accumulator tile goes
- * TMEM -> registers -> (dv, dmin, dmax) without ever materialising dWq.  Outputs are the PRE-sign
+ * dWq[N,K] = dYᵀ·X on wgmma with the qdq backward fused in the epilogue: the fp32 accumulator tile goes
+ * registers -> shared memory -> (dv, dmin, dmax) without ever materialising dWq.  Outputs are the PRE-sign
  * gradients (sign is taken after the cross-GPU all-reduce, auto_round/.../sign_sgd.py:389).
  * accumulate != 0 adds into dv/dmin/dmax (micro-batches / gradient_accumulate_steps).
  * dv_bf16 != 0: dv is bf16 [N,K] instead of fp32 (only the SIGN of the all-reduced sum is used by the update; bf16

@@ -1,31 +1,41 @@
-"""Differential fuzz of the oracle against the UNMODIFIED reference, live (build container only: /root/reference).
+"""Differential fuzz of the oracle against the UNMODIFIED reference (intel/auto-round v0.15.0).
 
 TEST INFRASTRUCTURE ONLY.  The committed fixtures under tests/golden/ pin the oracle on a fixed set of inputs; this script
-draws fresh random weights / rounding offsets / scales / importance vectors for many seeds and shapes and demands bit-exact
+draws seeded random weights / rounding offsets / scales / importance vectors for many seeds and shapes and demands bit-exact
 agreement of values AND autograd gradients between `oracle/qdq.py`, `oracle/pack.py` and the reference's registered
-functions and packers.  Run by tests/test_oracle_vs_reference_live.py in a subprocess (the import shim touches sys.path):
+functions and packers.  With the reference importable (`--record`, see oracle/ref_shim.py) it runs both sides and stores
+what the reference computed under tests/golden/: a canonical SHA-256 of every reference tensor (the comparison is bit-exact,
+so a digest decides it as well as the tensor would) and, for the loop replays, the recorded runs themselves.  Without
+`--record` the oracle side is checked against those stored results; tests/test_oracle_vs_reference_live.py runs it:
 
-    python -m oracle.diff_fuzz --seeds 8        -> prints one JSON line {"cases": N, "failures": [...]}
+    python -m oracle.diff_fuzz --seeds 6 [--record]     -> prints one JSON line {"cases": N, "failures": [...]}
+    python -m oracle.diff_fuzz --loops [--record]
 """
 from __future__ import annotations
 
 import argparse
+import hashlib
 import json
+import os
 import sys
 
 import torch
 
+GOLDEN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+DIGESTS = os.path.join(GOLDEN, "diff_fuzz_reference.json")
+LOOPS = os.path.join(GOLDEN, "diff_fuzz_loops.pt")
 
-def _same(a, b):
-    if a is None or b is None:
-        return a is None and b is None
-    a, b = a.detach(), b.detach()
-    if a.shape != b.shape:
-        a, b = a.reshape(-1), b.reshape(-1)
-        if a.shape != b.shape:
-            return False
-    nan = torch.isnan(a) & torch.isnan(b)
-    return bool(((a == b) | nan).all())
+
+def _digest(t):
+    """Canonical digest of a tensor's VALUES: float64, flat, -0.0 folded into +0.0, one NaN pattern -- equal digests iff
+    the values are equal element for element (NaN matching NaN), whatever the dtype or shape."""
+    if t is None:
+        return None
+    t = torch.as_tensor(t).detach().cpu()
+    t = t.view(torch.uint8) if t.dtype == torch.float8_e4m3fn else t
+    x = t.reshape(-1).to(torch.float64) + 0.0
+    x[torch.isnan(x)] = float("nan")
+    return hashlib.sha256(x.numpy().tobytes()).hexdigest()[:32]
 
 
 def _weights(n, k, gen, dtype=torch.bfloat16):
@@ -37,14 +47,25 @@ def _weights(n, k, gen, dtype=torch.bfloat16):
     return w
 
 
-def run(seeds: int):
-    from oracle.ref_shim import import_reference
-
-    import_reference()
-    from auto_round.data_type import QUANT_FUNC_WITH_DTYPE as REF
-    from auto_round.data_type.utils import reshape_pad_tensor_by_group_size
-
+def run(seeds: int, record: bool = False):
+    """record=True: run the reference live, compare, and return its digests; otherwise compare with the stored ones."""
     from oracle import qdq as Q
+
+    if record:
+        from oracle.ref_shim import import_reference
+
+        import_reference()
+        from auto_round.data_type import QUANT_FUNC_WITH_DTYPE as REF
+        ref_digests = {}
+    else:
+        REF = None
+        ref_digests = json.load(open(DIGESTS))
+
+    def check(key, ref_value, got):
+        """ref_value: a zero-argument callable computing the reference's tensor (only called when recording)."""
+        if record:
+            ref_digests[key] = _digest(ref_value())
+        return key in ref_digests and ref_digests[key] == _digest(got)
 
     failures, cases = [], 0
     shapes = [(8, 128), (5, 200), (16, 256), (3, 64)]
@@ -54,14 +75,14 @@ def run(seeds: int):
         for name, bits, g in (("int_sym", 4, 128), ("int_sym", 2, 32), ("int_sym", 3, 64), ("int_sym", 8, 32), ("int_asym", 2, 32),
                               ("int_asym", 4, 64), ("mx_fp4", 4, 32), ("nv_fp4", 4, 16)):
             w = _weights(n, k, gen)
-            grp, _, _ = reshape_pad_tensor_by_group_size(w, g)
+            grp, _, _ = Q.to_groups(w, g)
             G = grp.shape[0]
             v0 = (torch.rand(grp.shape, generator=gen) - 0.5).float()
             mn0 = (0.4 + 0.6 * torch.rand(G, generator=gen)).float()
             mx0 = (0.4 + 0.6 * torch.rand(G, generator=gen)).float()
             gq = torch.randn(w.shape, generator=gen).to(w.dtype)
             outs = []
-            for which in ("ref", "oracle"):
+            for which in (("ref", "oracle") if record else ("oracle",)):
                 v, mn, mx = (t.clone().requires_grad_(True) for t in (v0, mn0, mx0))
                 if name.startswith("int"):
                     wmin = torch.clamp(grp.min(1)[0], max=0)
@@ -87,8 +108,8 @@ def run(seeds: int):
                 outs.append((q, s, z if isinstance(z, torch.Tensor) else None, v.grad, mx.grad, mn.grad))
             cases += 1
             labels = ("qdq", "scale", "zp", "dV", "d max_scale", "d min_scale")
-            for lab, a, b in zip(labels, outs[0], outs[1]):
-                if not _same(a, b):
+            for i, (lab, b) in enumerate(zip(labels, outs[-1])):
+                if not check(f"fq/{seed}/{name}/w{bits}/g{g}/{lab}", lambda: outs[0][i], b):
                     failures.append(f"seed {seed} {name} w{bits} g{g} [{n}x{k}]: {lab} differs")
         # RTN variants and the optimized-RTN searches
         for name, bits, g in (("rtn_int_sym", 4, 128), ("opt_rtn_int_sym", 4, 32), ("opt_rtn_int_sym", 2, 32), ("opt_rtn_int_sym", 3, 128),
@@ -98,32 +119,47 @@ def run(seeds: int):
             if im is not None and seed % 5 == 0:
                 im[: max(1, k // 10)] = 0
             kw = dict(bits=bits, group_size=g)
+            a = None
             if name == "rtn_int_sym":
-                a = REF[name](w.clone(), **kw)
+                if record:
+                    a = REF[name](w.clone(), **kw)
                 b = Q.rtn_int_sym(w.clone(), bits, g)
             elif name == "opt_rtn_int_sym":
-                a = REF[name](w.clone(), imatrix=None if im is None else im.clone(), **kw)
+                if record:
+                    a = REF[name](w.clone(), imatrix=None if im is None else im.clone(), **kw)
                 b = Q.opt_rtn_int_sym(w.clone(), bits, g, im)
             elif name == "opt_rtn_nv_fp4":
                 gs = Q.nv_global_scale(w) * 0.9
-                a = REF[name](w.clone(), global_scale=gs, **({} if im is None else {"imatrix": im.clone()}), **kw)
+                if record:
+                    a = REF[name](w.clone(), global_scale=gs, **({} if im is None else {"imatrix": im.clone()}), **kw)
                 b = Q.opt_rtn_nv_fp4(w.clone(), 16, gs, 1.0, im)[:3]
             else:
-                a = REF[name](w.clone(), data_type="mx_fp4", imatrix=None if im is None else im.clone(), **kw)
+                if record:
+                    a = REF[name](w.clone(), data_type="mx_fp4", imatrix=None if im is None else im.clone(), **kw)
                 b = Q.opt_rtn_mx_fp4(w.clone(), 32, im)[:3]
             cases += 1
-            if not _same(a[0], b[0]):
+            key = f"rtn/{seed}/{name}/w{bits}/g{g}"
+            if not check(key + "/qdq", lambda: a[0], b[0]):
                 failures.append(f"seed {seed} {name} w{bits} g{g} [{n}x{k}] imatrix={'yes' if im is not None else 'no'}: qdq differs")
-            if not _same(a[1].float(), b[1].float()):
+            if not check(key + "/scale", lambda: a[1], b[1]):
                 failures.append(f"seed {seed} {name} w{bits} g{g} [{n}x{k}]: scale differs")
     # packers: reference QuantLinear.pack vs oracle/pack.py on fresh qdq weights (every bit of every buffer)
-    import numpy as np
     import torch.nn as nn
-    from auto_round.export.export_to_autoround.qlinear_fp import QuantLinear as FpQL
-    from auto_round_extension.torch.qlinear_torch import QuantLinear as PlainQL
-    from auto_round_extension.torch.qlinear_torch_zp import QuantLinear as ZpQL
 
     from oracle import pack as P
+
+    if record:
+        from auto_round.export.export_to_autoround.qlinear_fp import QuantLinear as FpQL
+        from auto_round_extension.torch.qlinear_torch import QuantLinear as PlainQL
+        from auto_round_extension.torch.qlinear_torch_zp import QuantLinear as ZpQL
+    else:
+        class _NoRef:                       # replay: the reference's packers are not called (check() never reads them)
+            def __init__(self, *a, **k):
+                self.device = None
+
+            def pack(self, *a, **k):
+                return None
+        FpQL = PlainQL = ZpQL = _NoRef
 
     def lin(wq):
         m = nn.Linear(wq.shape[1], wq.shape[0], bias=False)
@@ -132,9 +168,7 @@ def run(seeds: int):
 
     def cmp(tag, got: dict, ref_obj, keys):
         for key in keys:
-            r = getattr(ref_obj, key)
-            r = r.view(torch.uint8) if r.dtype == torch.float8_e4m3fn else r
-            if not np.array_equal(np.asarray(got[key]), r.numpy()):
+            if not check(f"pack/{tag}/{key}", lambda: getattr(ref_obj, key), got[key]):
                 failures.append(f"{tag}: packed buffer {key} differs")
 
     for seed in range(seeds):
@@ -170,17 +204,26 @@ def run(seeds: int):
         ql.pack(lin(wq), e.reshape(n, -1), device="cpu")
         cmp(f"seed {seed} pack mx_fp4", P.pack_mxfp4(wq, e.reshape(n, -1)), ql, ("weight_packed", "weight_scale"))
         cases += 2
+    if record:
+        with open(DIGESTS, "w") as f:
+            json.dump(ref_digests, f, indent=0, sort_keys=True)
     return {"cases": cases, "failures": failures}
 
 
-def run_loops():
+def run_loops(record: bool = False):
     """Whole tuning runs with NON-default loop options (the committed block fixtures all use the defaults): the reference's
-    AutoRound on the tiny Llama, recorded in memory by oracle/gen_golden.gen_block, replayed by oracle/signround.tune_block."""
-    from oracle.ref_shim import import_reference
-
-    import_reference()
-    import oracle.gen_golden as G
+    AutoRound on the tiny Llama, recorded by oracle/gen_golden.gen_block (record=True: live, and stored under tests/golden/),
+    replayed by oracle/signround.tune_block."""
     from oracle import signround as S
+
+    if record:
+        from oracle.ref_shim import import_reference
+
+        import_reference()
+        import oracle.gen_golden as G
+        recs = {}
+    else:
+        recs = torch.load(LOOPS, weights_only=False)
 
     configs = [
         ("minmax_off", dict(scheme="W4A16", group_size=32, enable_minmax_tuning=False), S.LayerScheme(4, 32, True, "int"),
@@ -197,7 +240,9 @@ def run_loops():
     failures, cases = [], 0
     for tag, kw, sc, okw in configs:
         bs = 2 if tag.endswith("bs2") else 4
-        rec = G.gen_block(tag, kw, iters=5, batch_size=bs, save=False)
+        if record:
+            recs[tag] = _compact(G.gen_block(tag, kw, iters=5, batch_size=bs, save=False))
+        rec = recs[tag]
         for bi, b in enumerate(rec["blocks"]):
             from oracle.tests_support import tiny_block
             blk = tiny_block(b["block_state"])
@@ -211,22 +256,42 @@ def run_loops():
             cases += 1
             if any(abs(a - e) > 1e-6 * abs(e) for a, e in zip(got, b["losses"])) or len(got) != len(b["losses"]):
                 failures.append(f"loop {tag} block {bi}: losses differ")
-            for name, lay in b["layers"].items():
-                if not torch.equal(blk.get_submodule(name).weight.data, lay["weight"]):
+            for name, digest in b["weight_digests"].items():
+                if _digest(blk.get_submodule(name).weight.data) != digest:
                     failures.append(f"loop {tag} block {bi}: final weight of {name} differs")
                     break
+    if record:
+        seen = {}
+
+        def dedup(o):                   # the runs share their inputs: store each distinct tensor once
+            if isinstance(o, torch.Tensor):
+                return seen.setdefault((o.dtype, tuple(o.shape), _digest(o)), o)
+            if isinstance(o, (list, tuple)):
+                return type(o)(dedup(v) for v in o)
+            return {k: dedup(v) for k, v in o.items()} if isinstance(o, dict) else o
+        torch.save(dedup(recs), LOOPS, _use_new_zipfile_serialization=False)
     return {"cases": cases, "failures": failures}
+
+
+def _compact(rec):
+    """What the replay reads of a recorded run: per block its inputs and the reference's losses, and a digest of every final
+    weight (compared bit for bit)."""
+    keep = ("block_state", "inputs", "others", "fp_outputs", "input_ids", "batches", "losses", "nv_gs")
+    blocks = [dict({k: b[k] for k in keep}, weight_digests={n: _digest(l["weight"]) for n, l in b["layers"].items()})
+              for b in rec["blocks"]]
+    return {"iters": rec["iters"], "blocks": blocks}
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--seeds", type=int, default=8)
     ap.add_argument("--loops", action="store_true", help="replay whole tuning runs with non-default loop options")
+    ap.add_argument("--record", action="store_true", help="run the reference live and store its results under tests/golden/")
     args = ap.parse_args()
     if args.loops:
-        res = run_loops()
+        res = run_loops(args.record)
         print(json.dumps(res))
         sys.exit(1 if res["failures"] else 0)
-    res = run(args.seeds)
+    res = run(args.seeds, args.record)
     print(json.dumps(res))
     sys.exit(1 if res["failures"] else 0)

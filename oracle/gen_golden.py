@@ -353,7 +353,7 @@ if __name__ == "__main__":
 # ---------------------------------------------------------------------------------------------
 # RTN + export fixture: the reference's own `iters=0, disable_opt_rtn=True` path through
 # quantize_and_save(format="auto_round") on the tiny Llama -> every packed tensor of the checkpoint.
-# Deterministic (no tuning), so the B200 path must reproduce the packed integers bit-for-bit.
+# Deterministic (no tuning), so the GPU path must reproduce the packed integers bit-for-bit.
 # ---------------------------------------------------------------------------------------------
 def gen_rtn_export(tag, scheme_kwargs, opt=False):
     import json

@@ -7,7 +7,7 @@ TEST INFRASTRUCTURE ONLY (see oracle/qdq.py header).  Restates, in plain torch o
     `_run_experts_with_routes`): loop over the experts, gather the (token, slot) pairs routed to each, run its three
     linears, scale by the routing weight, sum the k slots per token.
 Used by tests/test_oracle_golden.py to replay a reference Mixtral tuning run bit-for-bit (tests/golden/block_mixtral_mxfp4.pt)
-and by the GPU parity tests as the reference the product's grouped tcgen05 path (auto_round_b200/moe.py) is checked against.
+and by the GPU parity tests as the reference the product's grouped wgmma path (auto_round_b200/moe.py) is checked against.
 The product never imports this module."""
 import torch
 import torch.nn as nn

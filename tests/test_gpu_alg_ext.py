@@ -1,7 +1,6 @@
 """enable_alg_ext on the GPU (SURVEY.md 8 rows a10 / a19): searched init scale, max_scale in [0, 2], outlier-suppressed loss.
 
-First run on a B200 in round 2 (gpurun_out/r2_gated_all.log -> profiles/r02_gated_modules.txt): all green once the
-all-zero-group NaN of the reference's autograd (DESIGN.md 5b #2) is masked in the comparison.
+The all-zero-group NaN of the reference's autograd (DESIGN.md 5b #2) is masked in the comparison.
 
 What they state (same bars as tests/test_gpu_kernels.py / test_gpu_engine.py):
   * fake-quant forward with an init scale: bit-exact to the oracle (int sym, MXFP4, NVFP4)

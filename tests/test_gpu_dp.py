@@ -5,7 +5,7 @@ Two transports for the same code path (quantizer.quantize_block with DataParalle
     reduce-scatter of the bf16 dWq (emulated), row-sharded fused update (ar_fq_update rows [r0, r1)), all-gather of the
     new fake-quant weight and of the best-parameter shards, global loss for the best-iteration choice;
   * `nccl`, one rank per GPU, iteration captured as a CUDA graph with the collectives inside -- needs >= 2 GPUs
-    (`gpurun --gpus 2`; skipped on a single-GPU box).
+    (skipped on a single-GPU machine).
 What is compared (the sum over ranks of bf16-rounded partial gradients is not the bf16 rounding of the total, so sign flips on
 ~zero gradients make the trajectories differ; SURVEY.md 8d bars):
   * both ranks end with bit-identical weights / scales (no broadcast is needed);
@@ -177,7 +177,7 @@ def test_two_ranks_one_gpu_gloo_equals_one_rank(tag, tmp_path):
     _check(tag, "gloo", tmp_path)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="one rank per GPU over NCCL needs >= 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="one rank per GPU over NCCL needs >= 2 GPUs")
 @pytest.mark.parametrize("tag", ["w4a16_sym_g32", "algext_w2a16_sym_g32", "mixtral_mxfp4"])
 def test_two_ranks_nccl_graph_equals_one_rank(tag, tmp_path):
     _check(tag, "nccl", tmp_path)

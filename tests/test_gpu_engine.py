@@ -1,7 +1,7 @@
 """GPU parity of the tuning engine (quantize_block / AutoRound) against the reference fixtures and the CPU oracle.
 
 The sign-SGD trajectory is chaotic (sign flips on tiny gradients; bf16 GEMM summation order differs between
-cuBLAS-on-CPU/oneDNN and tcgen05), so loop-level parity is stated as (SURVEY.md 8d):
+cuBLAS-on-CPU/oneDNN and wgmma), so loop-level parity is stated as (SURVEY.md 8d):
   (ii)  iteration-0 loss per block (V=0: pure RTN forward):           |rel err| <= 2e-2 on tiny blocks
         (bf16 activations of a 64-wide block: one bf16 ulp of the output is already 4e-3 of the error signal)
   (iii) sign(dV) agreement with the oracle's autograd at iteration 0:  >= 97 % on elements above the noise floor

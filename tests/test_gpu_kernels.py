@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle and the committed golden
-fixtures of the reference.  Run on the B200 box:  python -m pytest tests -m gpu -q
+fixtures of the reference.  Run on an H100:  python -m pytest tests -m gpu -q
 
 Tolerances (stated per check):
   * integer / byte outputs (packed words, codes, nibbles, e4m3/e8m0 scales): bit-exact;

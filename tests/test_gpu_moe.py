@@ -1,4 +1,4 @@
-"""GPU parity of the MoE path (SURVEY.md 8 f2): device-side routing, grouped tcgen05 GEMMs and the combine kernels of
+"""GPU parity of the MoE path (SURVEY.md 8 f2): device-side routing, grouped wgmma GEMMs and the combine kernels of
 auto_round_b200/moe.py against the reference's expert loop restated in oracle/moe_loop.py (auto_round/modeling/fused_moe/
 moe_experts_interface.py:173-260), and a whole Mixtral block tuned against the oracle on the reference's own fixture."""
 import copy
@@ -147,7 +147,7 @@ def _mixtral_block(state, grouped: bool, device):
 
 
 def test_mixtral_block_vs_oracle(golden_dir):
-    """BASELINE.json config 5's scheme (MXFP4 weight-only) on the reference's tiny 4-expert Mixtral fixture: grouped tcgen05
+    """BASELINE.json config 5's scheme (MXFP4 weight-only) on the reference's tiny 4-expert Mixtral fixture: grouped wgmma
     path + CUDA graph vs the oracle loop, same batches (bars of tests/test_gpu_engine.py).  The oracle (plain torch) runs on
     the GPU here: top-2 routing is discontinuous, and the router's bf16 GEMM on the CPU sends 1 of the fixture's 64 tokens to
     another expert than the same GEMM on the GPU, which alone moves the loss by 7 % (tools/diag_moe.py: oracle-CPU 3.12e-6,

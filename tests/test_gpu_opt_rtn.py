@@ -187,7 +187,7 @@ def test_default_rtn_checkpoint_matches_reference(golden_dir, tag, tmp_path):
         a, b = got[k].contiguous().view(torch.uint8).reshape(-1), ref.contiguous().view(torch.uint8).reshape(-1)
         frac = (a != b).float().mean().item()
         worst = max(worst, frac)
-        assert frac <= (0.0 if tag == "opt_mxfp4" else 0.02), (k, frac)      # measured on B200: 0.00195
+        assert frac <= (0.0 if tag == "opt_mxfp4" else 0.02), (k, frac)
     print(f"{tag}: worst mismatching byte fraction {worst:.5f}")
     extra = {k for k in got if ".layers." in k and "layernorm" not in k} - set(rec["tensors"])
     assert not extra, extra

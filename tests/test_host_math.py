@@ -1,7 +1,7 @@
 """CPU tier: the PRODUCT's device math (auto_round_b200/csrc/ar_qdq_math.cuh -- the struct every CUDA kernel and the fused
 GEMM epilogue call) compiled as host C++ (tests/host_math/math_host.cpp, g++) and checked against the oracle.
 
-This does not replace the GPU parity tests (the kernels' indexing, reductions and launches only run on a B200); it pins the
+This does not replace the GPU parity tests (the kernels' indexing, reductions and launches only run on the GPU); it pins the
 formulas themselves without a GPU -- in particular the enable_alg_ext `init_scale` branches written after round 1's GPU
 budget was spent."""
 import ctypes as C

@@ -298,7 +298,7 @@ def test_tune_block_mixtral_moe_matches_reference_bit_exact(golden_dir):
     expert parameters into per-expert linears (modeling/fused_moe/moe_experts_interface.py:173-260).  The block here is built
     with the oracle's restatement of that un-fusing and expert loop (oracle/moe_loop.py), so a bit-exact replay of the
     reference's 8 iterations pins it and the oracle loop on ragged expert batches (experts that see no token get no update);
-    the product's grouped tcgen05 path (auto_round_b200/moe.py) is checked against it on the GPU (tests/test_gpu_moe.py)."""
+    the product's grouped wgmma path (auto_round_b200/moe.py) is checked against it on the GPU (tests/test_gpu_moe.py)."""
     from transformers import MixtralConfig
     from transformers.models.mixtral.modeling_mixtral import MixtralDecoderLayer
 

@@ -1,4 +1,4 @@
-"""One-shot GPU diagnostics (run under gpurun): correctness of every GEMM variant + timing vs cuBLAS.
+"""One-shot GPU diagnostics (run on a GPU machine): correctness of every GEMM variant + timing vs cuBLAS.
 Writes gpurun_out/diag.json.  Not a test and not the bench: a development probe."""
 import json
 import os
