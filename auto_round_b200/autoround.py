@@ -26,7 +26,7 @@ from . import export, ops
 from . import resume as resume_mod
 from .fused import fused_block_ops
 from .moe import unfuse_experts
-from .quantizer import DataParallel, SignRoundQuantizer
+from .quantizer import DataParallel, SignRoundQuantizer, valid_token_masks
 from .schemes import QuantizationScheme, parse_scheme
 from .wrapper import set_module
 
@@ -58,6 +58,29 @@ def find_blocks(model: nn.Module):
             if any(isinstance(sub, nn.Linear) for sub in mod[0].modules()):
                 return name, mod
     raise RuntimeError("no transformer block list found in the model")
+
+
+def repeated_tail(input_ids: torch.Tensor) -> torch.Tensor:
+    """bool [b, s]: in each row, the run of positions just before the last one that hold the row's last token.  Without
+    a pad token the reference takes that run for padding (calibration/llm.py:351-358, :375-389)."""
+    same = input_ids[:, :-1] == input_ids[:, -1:]
+    run = same.flip(1).cumprod(1).flip(1).bool()              # stays true back from the end until the first other token
+    return torch.cat([run, run.new_zeros(run.shape[0], 1)], dim=1)
+
+
+def label_ids_and_mask(input_ids: torch.Tensor, tokenizer):
+    """One token batch [b, s] -> (label ids with -100 at every position excluded from the loss, long attention mask), the
+    reference's conventions for tensor datasets (calibration/llm.py:346-398).  Padding is the pad id, or the repeated
+    tail when the tokenizer has no pad id (labels) or no pad token (mask); the last position is always excluded."""
+    pad_id = getattr(tokenizer, "pad_token_id", None)
+    ids = input_ids.masked_fill((input_ids == pad_id) if pad_id is not None else repeated_tail(input_ids), -100)
+    ids[:, -1] = -100
+    if pad_id is not None and getattr(tokenizer, "pad_token", None) is not None:
+        am = (input_ids != pad_id).to(torch.long)
+    else:
+        am = (~repeated_tail(input_ids)).to(torch.long)
+    am[:, -1] = 0
+    return ids, am
 
 
 class _GemmLinear(nn.Module):
@@ -226,6 +249,7 @@ class AutoRound:
         self.timings = {}
         self._pack_on_the_fly = False
         self._packed = False
+        self._lm_head_extra = None              # {name: extra_config entry} of layers quantized outside the blocks
 
     # -------------------------------------------------------------------------------------------
     @staticmethod
@@ -308,9 +332,6 @@ class AutoRound:
         blocks = getattr(self, "_blocks", None)
         if blocks is None:
             _, blocks = find_blocks(model)
-        moved = []
-        for name, mod in model.named_children():
-            moved.append(mod)
         block_ids = {id(b) for b in blocks}
         for mod in model.modules():
             if id(mod) in block_ids:
@@ -325,34 +346,8 @@ class AutoRound:
         try:
             for data in self._token_batches():
                 input_ids = data.to(dev)
-                ids = input_ids.clone()
-                pad_id = getattr(self.tokenizer, "pad_token_id", None)
-                if pad_id is not None:
-                    ids[ids == pad_id] = -100
-                else:
-                    for b in range(ids.shape[0]):
-                        last = ids[b, -1].clone()
-                        j = ids.shape[1] - 2
-                        while j >= 0 and ids[b, j] == last:
-                            ids[b, j] = -100
-                            j -= 1
-                ids[:, -1] = -100
+                ids, am = label_ids_and_mask(input_ids, self.tokenizer)
                 ids_cache.extend(torch.split(ids.cpu(), 1, dim=0))
-                if pad_id is not None and getattr(self.tokenizer, "pad_token", None) is not None:
-                    am = (input_ids != pad_id).to(torch.long)
-                else:
-                    am = torch.ones_like(input_ids, dtype=torch.long)
-                    for b in range(input_ids.shape[0]):
-                        last = input_ids[b, -1]
-                        j = input_ids.shape[1] - 2
-                        rep = False
-                        while j >= 0 and input_ids[b, j] == last:
-                            rep = True
-                            am[b, j] = 0
-                            j -= 1
-                        if rep:
-                            am[b, -1] = 0
-                am[:, -1] = 0
                 try:
                     with torch.autocast(device_type="cuda", dtype=self.amp_dtype):
                         model(input_ids, attention_mask=am, use_cache=False)
@@ -448,30 +443,34 @@ class AutoRound:
 
     # ---------------------------------------------------------------------------------- quantize
     def quantize(self):
+        """Quantize the blocks one after the other.  `iters > 0` tunes every block with SignRound; `iters == 0` runs the
+        RTN mode `_rtn_mode` selects.  Tuning and the calibrated optimized RTN cache the first block's inputs once and
+        feed each block's full-precision outputs to the next one."""
         model = self.model
         prefix, blocks = find_blocks(model)
         self.block_prefix, self._blocks = prefix, blocks
-        if self.iters == 0:
-            mode = self._rtn_mode()
-            return self._quantize_opt_rtn(prefix, blocks) if mode == "calibrated_opt" else self._quantize_rtn(prefix, blocks, mode)
-        t_cache0 = time.time()
-        fp_inputs, others, ids_cache = self.cache_block_inputs(blocks[0])
-        torch.cuda.synchronize(self.device)
-        self.timings["cache_inputs_s"] = time.time() - t_cache0
-        token_masks_cpu = [(ids != -100).reshape(-1) for ids in ids_cache]
-        any_masked = not all(bool(m.all()) for m in token_masks_cpu)
-        token_masks = [m.to(self.device) for m in token_masks_cpu] if any_masked else None
+        mode = "tune" if self.iters > 0 else self._rtn_mode()
+        tune = mode == "tune"
+        fp_inputs = others = ids_cache = token_masks = None
+        if mode in ("tune", "calibrated_opt"):
+            t_cache0 = time.time()
+            fp_inputs, others, ids_cache = self.cache_block_inputs(blocks[0])
+            if tune:
+                torch.cuda.synchronize(self.device)
+                self.timings["cache_inputs_s"] = time.time() - t_cache0
+            token_masks = valid_token_masks(ids_cache, self.device)
 
+        tune_kw = dict(enable_alg_ext=self.enable_alg_ext, gradient_accumulate_steps=self.gradient_accumulate_steps,
+                       **self.sign_kw) if tune else {}                    # RTN ignores the tuning options
         quantizer = SignRoundQuantizer(self.scheme, iters=self.iters, batch_size=self.batch_size, amp_dtype=self.amp_dtype,
-                                       layer_config=self.layer_config, dp=self.dp, enable_alg_ext=self.enable_alg_ext,
-                                       gradient_accumulate_steps=self.gradient_accumulate_steps, **self.sign_kw)
+                                       layer_config=self.layer_config, dp=self.dp, **tune_kw)
         self.quantizer = quantizer
         t0 = time.time()                                                  # orchestrator.py:631
         q_inputs = None
         nblk = len(blocks)
         # AR_RESUME_DIR (utils/resume.py, orchestrator.py:634-676): skip the blocks a previous process finished, restore
         # their results and the two chain values, and persist the same after every block of this run
-        resume, start = self._open_resume(prefix, blocks)
+        resume, start = self._open_resume(prefix, blocks) if tune else (None, 0)
         if resume is not None and start > 0:
             fp_chain, q_chain, rng = resume.load_input_ids(), resume.load_q_input(), None
             if fp_chain is None:
@@ -481,10 +480,7 @@ class AutoRound:
                 rng = snap.pop("__rng__", rng)
                 quantizer.block_prefix = f"{prefix}.{bj}"
                 unfuse_experts(blocks[bj])                                # snapshots hold per-expert names
-                for p in blocks[bj].parameters():                         # same normalisation as the live path
-                    p.requires_grad_(False)
-                    if p.dtype in (torch.float32, torch.float16):
-                        p.data = p.data.to(self.amp_dtype)
+                self._freeze(blocks[bj])                                  # same normalisation as the live path
                 resume_mod.restore_block(blocks[bj], snap, quantizer.scheme_for)
                 self.block_results.append({"block": f"{prefix}.{bj}", "resumed": True})
             fp_inputs = [t.to(self.device) for t in fp_chain]
@@ -492,6 +488,10 @@ class AutoRound:
             if rng is not None:                                           # the sampler continues where the dead run was
                 random.setstate(rng["python"])
                 torch.set_rng_state(rng["torch"])
+        # The zero-shot RTN modes list every linear the layer filter accepts, so there a layer that layer_config lifts
+        # above 8 bits still joins the shared NVFP4 global scale of its q/k/v or gate/up group; the calibrated modes
+        # list only the layers they quantize.
+        all_linears = mode in ("plain", "zero_shot_opt")
         for bi, block in enumerate(blocks):
             if bi < start:
                 continue
@@ -500,62 +500,81 @@ class AutoRound:
             self._hook(bi, "h2d0")
             block.to(self.device)                                         # H2D of this block's weights
             unfuse_experts(block)                                         # MoE: fused 3-D experts -> per-expert nn.Linear
-            for p in block.parameters():
-                p.requires_grad_(False)
-                if p.dtype in (torch.float32, torch.float16):
-                    p.data = p.data.to(self.amp_dtype)
+            self._freeze(block)
             self._hook(bi, "compute0")
-            names = [n for n, m in block.named_modules() if quantizer.layer_filter(n, m)
-                     and (quantizer.scheme_for(n, m) is not None) and quantizer.scheme_for(n, m).bits <= 8]
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
-            ev[0].record()
-            # (3) reference outputs of the FP block on the FP inputs  (composer.py:423-429)
-            imatrices = None
-            if self.enable_alg_ext and self.scheme.qdq_name != "int_asym":   # imatrix hooks on the FP-input forward, raw
-                # sums (sign_roundv2/quantizer.py:401-428); the reference collects them for asym too but never reads them
-                with _collect_imatrix(block, names, self.device) as col:
-                    ref_out = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
-                imatrices = col.finish(self.dp, normalise=False)
-            else:
-                ref_out = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
-            ev[1].record()
+            names = [n for n, m in block.named_modules() if quantizer.layer_filter(n, m) and (all_linears or (
+                     quantizer.scheme_for(n, m) is not None and quantizer.scheme_for(n, m).bits <= 8))]
             nv_gs = self._fuse_nv_global_scales(block, names) if self.scheme.qdq_name == "nv_fp4" else None
-            eff = q_inputs if (q_inputs is not None and quantizer.enable_quanted_input) else fp_inputs
-            quantizer.quantize_block(block, eff, others, ref_out, q_inputs, None, input_ids=ids_cache,
-                                     nv_global_scales=nv_gs, imatrices=imatrices)
-            res = quantizer.last_result
-            ev[2].record()
-            # (6) outputs of the quantised block feed the next block (composer.py:476-481)
-            if quantizer.enable_quanted_input and (bi + 1 < nblk or self.quant_lm_head):
-                q_inputs = self._forward_all(quantizer, block, eff, others, token_masks)
+            if tune:
+                ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+                ev[0].record()
+                # (3) reference outputs of the FP block on the FP inputs  (composer.py:423-429)
+                imatrices = None
+                if self.enable_alg_ext and self.scheme.qdq_name != "int_asym":   # imatrix hooks on the FP-input forward,
+                    # raw sums (sign_roundv2/quantizer.py:401-428); the reference collects them for asym too but never reads them
+                    with _collect_imatrix(block, names, self.device) as col:
+                        ref_out = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
+                    imatrices = col.finish(self.dp, normalise=False)
+                else:
+                    ref_out = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
+                ev[1].record()
+                eff = q_inputs if (q_inputs is not None and quantizer.enable_quanted_input) else fp_inputs
+                quantizer.quantize_block(block, eff, others, ref_out, q_inputs, None, input_ids=ids_cache,
+                                         nv_global_scales=nv_gs, imatrices=imatrices)
+                res = quantizer.last_result
+                done = res.quantized_layers
+                ev[2].record()
+                # (6) outputs of the quantised block feed the next block (composer.py:476-481)
+                if quantizer.enable_quanted_input and (bi + 1 < nblk or self.quant_lm_head):
+                    q_inputs = self._forward_all(quantizer, block, eff, others, token_masks)
+                else:
+                    q_inputs = None
+                # per-block output MSE of the tuned block against the FP block over ALL samples (valid tokens only) -- the
+                # second half of the headline metric; a device scalar, read back after the last block (no host sync here)
+                blk_mse = self._block_mse(q_inputs, ref_out, token_masks) if q_inputs is not None else None
+                fp_inputs = ref_out
+                ev[3].record()
             else:
-                q_inputs = None
-            # per-block output MSE of the tuned block against the FP block over ALL samples (valid tokens only) -- the second
-            # half of the headline metric; a device scalar, read back after the last block (no host sync here)
-            blk_mse = self._block_mse(q_inputs, ref_out, token_masks) if q_inputs is not None else None
-            fp_inputs = ref_out
-            ev[3].record()
+                # OptimizedRTNQuantizer (rtn/quantizer.py:72-140): the FP forward over the calibration set collects each
+                # linear's importance (sum x^2 per input channel / #samples) for the weighted scale search; iters == 0
+                # implies enable_quanted_input=False, so the FP outputs feed the next block (composer.py:423-429, 476-483)
+                imatrices = {} if mode == "zero_shot_opt" else None
+                if mode == "calibrated_opt":
+                    with _collect_imatrix(block, names, self.device) as col:
+                        fp_inputs = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
+                    imatrices = col.finish(self.dp, normalise=True)
+                done = quantizer.rtn_block(block, None, nv_gs, imatrices=imatrices,
+                                           is_moe=any("experts" in n for n in names))
             if self._pack_on_the_fly:                                     # immediate_pack (orchestrator.py:327-337)
-                for n in res.quantized_layers:
+                for n in done:
                     export.pack_layer(n, block, quantizer.scheme_for(n, block.get_submodule(n)), self.device,
                                       out_device=self.device)
-            ev[4].record()
+            if tune:
+                ev[4].record()
             self._hook(bi, "d2h0")
             block.to("cpu")                                               # packed tensors (or qdq weights) -> host
             self._hook(bi, "done")
-            torch.cuda.synchronize(self.device)
-            if resume is not None and self.dp.rank == 0:                  # one writer; every rank holds identical results
-                snap = resume_mod.snapshot_block(block)
-                snap["__rng__"] = {"python": random.getstate(), "torch": torch.get_rng_state()}
-                resume.mark_block_done(f"{prefix}.{bi}", snap, q_inputs, fp_inputs)
-            phases = {k: ev[i].elapsed_time(ev[i + 1]) for i, k in enumerate(("ref_forward_ms", "tune_ms", "q_forward_ms", "pack_ms"))}
-            self.block_results.append({"block": f"{prefix}.{bi}", "init_loss": res.init_loss, "best_loss": res.best_loss,
-                                       "best_iter": res.best_iter, "seconds": time.time() - tb, "losses": res.losses,
-                                       "phases_ms": phases, "cuda_graph": res.used_cuda_graph, "batches": res.batches,
-                                       "block_mse": blk_mse})
-        self._lm_head_extra = None
-        if self.quant_lm_head:
+            if tune:
+                torch.cuda.synchronize(self.device)
+                if resume is not None and self.dp.rank == 0:              # one writer; every rank holds identical results
+                    snap = resume_mod.snapshot_block(block)
+                    snap["__rng__"] = {"python": random.getstate(), "torch": torch.get_rng_state()}
+                    resume.mark_block_done(f"{prefix}.{bi}", snap, q_inputs, fp_inputs)
+                phases = {k: ev[i].elapsed_time(ev[i + 1])
+                          for i, k in enumerate(("ref_forward_ms", "tune_ms", "q_forward_ms", "pack_ms"))}
+                self.block_results.append({"block": f"{prefix}.{bi}", "init_loss": res.init_loss, "best_loss": res.best_loss,
+                                           "best_iter": res.best_iter, "seconds": time.time() - tb, "losses": res.losses,
+                                           "phases_ms": phases, "cuda_graph": res.used_cuda_graph, "batches": res.batches,
+                                           "block_mse": blk_mse})
+            elif mode == "calibrated_opt":
+                rec = {"block": f"{prefix}.{bi}", "imatrix_layers": len(imatrices)}
+                if getattr(self, "keep_imatrix", False):                  # inspection hook for the parity tests
+                    rec["imatrix"] = {n: (None if t is None else t.detach().cpu()) for n, t in imatrices.items()}
+                self.block_results.append(rec)
+        if tune and self.quant_lm_head:
             self._quantize_lm_head(quantizer, fp_inputs, q_inputs, ids_cache)
+        if not tune:
+            torch.cuda.synchronize(self.device)                           # the RTN loop never waits on the device
         self.timings["tuning_s"] = time.time() - t0                      # "quantization tuning time" (orchestrator.py:792)
         for r in self.block_results:                                      # device scalars -> python floats
             if isinstance(r.get("block_mse"), torch.Tensor):
@@ -564,15 +583,34 @@ class AutoRound:
             resume.clear()                                                # a finished run leaves no state behind
         self.quantized = True
         self._packed = self._pack_on_the_fly
-        self.block_prefix = prefix
         layer_cfg = {}
-        for bi, block in enumerate(blocks):
-            quantizer.block_prefix = f"{prefix}.{bi}"
-            for n, m in block.named_modules():
-                if hasattr(m, "scale") or isinstance(m, export.QuantLinear):
-                    layer_cfg[f"{prefix}.{bi}.{n}"] = quantizer.scheme_for(n, m).to_dict()
+        if tune:                                                          # the RTN modes report no per-layer config
+            quantized = lambda m: hasattr(m, "scale") or isinstance(m, export.QuantLinear)    # noqa: E731
+            layer_cfg = {full: sc.to_dict() for _, _, full, sc in self._block_layers(quantized)}
         self.layer_config_out = layer_cfg
         return model, layer_cfg
+
+    def _freeze(self, *modules: nn.Module):
+        """Prepare modules for quantization: no autograd on their parameters, fp32/fp16 parameters cast to the amp dtype."""
+        for mod in modules:
+            for p in mod.parameters():
+                p.requires_grad_(False)
+                if p.dtype in (torch.float32, torch.float16):
+                    p.data = p.data.to(self.amp_dtype)
+
+    def _block_layers(self, keep):
+        """(block, block-relative name, full name, resolved scheme) of every module of every block that `keep(module)`
+        accepts.  While a block is walked `quantizer.block_prefix` names it, so that layer_config keys given as full
+        module names resolve; the walk clears it at the end.  Modules may be replaced while the walk is suspended."""
+        q = self.quantizer
+        try:
+            for bi, block in enumerate(self._blocks):
+                q.block_prefix = f"{self.block_prefix}.{bi}"
+                for n, m in list(block.named_modules()):
+                    if keep(m):
+                        yield block, n, f"{q.block_prefix}.{n}", q.scheme_for(n, m)
+        finally:
+            q.block_prefix = None
 
     def _find_tail(self):
         """(final norm module, output projection, its name) of a causal LM: the layers between the last block and the
@@ -597,10 +635,7 @@ class AutoRound:
         quantizer.block_prefix = None                 # `name` is already a full module name
         norm.to(self.device)
         head.to(self.device)
-        for p in list(norm.parameters()) + list(head.parameters()):
-            p.requires_grad_(False)
-            if p.dtype in (torch.float32, torch.float16):
-                p.data = p.data.to(self.amp_dtype)
+        self._freeze(norm, head)
         with torch.no_grad(), torch.autocast(device_type="cuda", dtype=self.amp_dtype):
             fp_h = [norm(t.to(self.device)).to(self.amp_dtype) for t in fp_chain]
             q_h = None if q_chain is None else [norm(t.to(self.device)).to(self.amp_dtype) for t in q_chain]
@@ -650,116 +685,27 @@ class AutoRound:
             return "calibrated_opt"
         return "calibrated_opt" if name == "nv_fp4" else "zero_shot_opt"
 
-    def _quantize_rtn(self, prefix, blocks, mode: str = "plain"):
-        """iters == 0, zero-shot (orchestrator.py:420 "Zero-shot mode"): block by block, no calibration data; `mode` is
-        "plain" or "zero_shot_opt" (see _rtn_mode).  The calibrated route is `_quantize_opt_rtn`."""
-        quantizer = SignRoundQuantizer(self.scheme, iters=0, batch_size=self.batch_size, amp_dtype=self.amp_dtype,
-                                       layer_config=self.layer_config, dp=self.dp)
-        self.quantizer = quantizer
-        t0 = time.time()
-        for bi, block in enumerate(blocks):
-            quantizer.block_prefix = f"{prefix}.{bi}"
-            self._hook(bi, "h2d0")
-            block.to(self.device)
-            unfuse_experts(block)
-            for p in block.parameters():
-                p.requires_grad_(False)
-                if p.dtype in (torch.float32, torch.float16):
-                    p.data = p.data.to(self.amp_dtype)
-            self._hook(bi, "compute0")
-            names = [n for n, m in block.named_modules() if quantizer.layer_filter(n, m)]
-            nv_gs = self._fuse_nv_global_scales(block, names) if self.scheme.qdq_name == "nv_fp4" else None
-            done = quantizer.rtn_block(block, None, nv_gs, imatrices=({} if mode == "zero_shot_opt" else None),
-                                       is_moe=any("experts" in n for n in names))
-            if self._pack_on_the_fly:
-                for n in done:
-                    export.pack_layer(n, block, quantizer.scheme_for(n, block.get_submodule(n)), self.device,
-                                      out_device=self.device)
-            self._hook(bi, "d2h0")
-            block.to("cpu")
-            self._hook(bi, "done")
-        torch.cuda.synchronize(self.device)
-        self.timings["tuning_s"] = time.time() - t0
-        self.quantized, self._packed = True, self._pack_on_the_fly
-        self.layer_config_out = {}
-        return self.model, self.layer_config_out
-
-    def _quantize_opt_rtn(self, prefix, blocks):
-        """iters == 0, `disable_opt_rtn` unset -- the reference's default RTN (OptimizedRTNQuantizer,
-        algorithms/quantization/rtn/quantizer.py:72-140): per block, the full-precision forward over the calibration set
-        collects each linear's importance matrix (sum x^2 per input channel / #samples), then every layer's scale comes
-        from the importance-weighted grid search (ar_search_scale_*).  iters == 0 implies enable_quanted_input=False, so the
-        next block is fed the full-precision outputs (composer.py:423-429, 476-483)."""
-        fp_inputs, others, ids_cache = self.cache_block_inputs(blocks[0])
-        token_masks_cpu = [(ids != -100).reshape(-1) for ids in ids_cache]
-        any_masked = not all(bool(m.all()) for m in token_masks_cpu)
-        token_masks = [m.to(self.device) for m in token_masks_cpu] if any_masked else None
-        quantizer = SignRoundQuantizer(self.scheme, iters=0, batch_size=self.batch_size, amp_dtype=self.amp_dtype,
-                                       layer_config=self.layer_config, dp=self.dp)
-        self.quantizer = quantizer
-        t0 = time.time()
-        for bi, block in enumerate(blocks):
-            quantizer.block_prefix = f"{prefix}.{bi}"
-            self._hook(bi, "h2d0")
-            block.to(self.device)
-            unfuse_experts(block)
-            for p in block.parameters():
-                p.requires_grad_(False)
-                if p.dtype in (torch.float32, torch.float16):
-                    p.data = p.data.to(self.amp_dtype)
-            self._hook(bi, "compute0")
-            names = [n for n, m in block.named_modules() if quantizer.layer_filter(n, m)
-                     and (quantizer.scheme_for(n, m) is not None) and quantizer.scheme_for(n, m).bits <= 8]
-            is_moe = any("experts" in n for n in names)
-            with _collect_imatrix(block, names, self.device) as col:
-                ref_out = self._forward_all(quantizer, block, fp_inputs, others, token_masks)
-            imatrices = col.finish(self.dp, normalise=True)
-            nv_gs = self._fuse_nv_global_scales(block, names) if self.scheme.qdq_name == "nv_fp4" else None
-            done = quantizer.rtn_block(block, None, nv_gs, imatrices=imatrices, is_moe=is_moe)
-            if self._pack_on_the_fly:
-                for n in done:
-                    export.pack_layer(n, block, quantizer.scheme_for(n, block.get_submodule(n)), self.device,
-                                      out_device=self.device)
-            fp_inputs = ref_out
-            self._hook(bi, "d2h0")
-            block.to("cpu")
-            self._hook(bi, "done")
-            rec = {"block": f"{prefix}.{bi}", "imatrix_layers": len(imatrices)}
-            if getattr(self, "keep_imatrix", False):           # inspection hook for the parity tests
-                rec["imatrix"] = {n: (None if t is None else t.detach().cpu()) for n, t in imatrices.items()}
-            self.block_results.append(rec)
-        torch.cuda.synchronize(self.device)
-        self.timings["tuning_s"] = time.time() - t0
-        self.quantized, self._packed = True, self._pack_on_the_fly
-        self.layer_config_out = {}
-        return self.model, self.layer_config_out
-
     def save_quantized(self, output_dir: Optional[str] = None, format: str = "auto_round", inplace: bool = True):
         if format not in ("auto_round", "auto_round:auto_gptq"):
             raise NotImplementedError(f"format {format!r}: only the auto_round checkpoint format is in scope")
         if not self.quantized:
             raise RuntimeError("call quantize() first")
-        prefix, blocks = self.block_prefix, self._blocks
         if not self._packed:
-            for bi, block in enumerate(blocks):
-                self.quantizer.block_prefix = f"{prefix}.{bi}"
-                for n, m in list(block.named_modules()):
-                    if type(m) is nn.Linear and hasattr(m, "scale"):
-                        export.pack_layer(n, block, self.quantizer.scheme_for(n, m), self.device)
-            self.quantizer.block_prefix = None
-            for n in (getattr(self, "_lm_head_extra", None) or {}):        # layers tuned outside the blocks (lm_head)
+            for block, n, _, sc in self._block_layers(lambda m: type(m) is nn.Linear and hasattr(m, "scale")):
+                export.pack_layer(n, block, sc, self.device)
+            for n in (self._lm_head_extra or {}):                           # layers tuned outside the blocks (lm_head)
                 m = self.model.get_submodule(n)
                 if type(m) is nn.Linear and hasattr(m, "scale"):
                     export.pack_layer(n, self.model, self.quantizer.scheme_for(n, m), self.device)
             self._packed = True
-        extra = dict(getattr(self, "_lm_head_extra", None) or {})
-        extra.update(self._layer_config_overrides(prefix, blocks))
+        extra = dict(self._lm_head_extra or {})
+        extra.update(self._layer_config_overrides())
         tuning = dict(self.sign_kw)
         lr_used = self.quantizer.compute_lr(self.scheme.bits) if self.iters > 0 else None
         if lr_used is not None and "lr" not in tuning and lr_used != 1.0 / self.iters:
             tuning["lr"] = lr_used                    # the auto rule gave 2/iters: the reference serialises the resolved lr
             tuning.setdefault("minmax_lr", lr_used)
-        qcfg = export.build_quantization_config(self.scheme, prefix, extra or None, self.iters,
+        qcfg = export.build_quantization_config(self.scheme, self.block_prefix, extra or None, self.iters,
                                                 self.nsamples, self.seqlen, self.batch_size, tuning=tuning)
         self.quantization_config = qcfg
         if output_dir is None:
@@ -768,24 +714,19 @@ class AutoRound:
         export.save_quantized(self.model, output_dir, qcfg, self.tokenizer)
         return self.model
 
-    def _layer_config_overrides(self, prefix, blocks) -> dict:
+    def _layer_config_overrides(self) -> dict:
         """`extra_config` entries for block layers whose resolved scheme differs from the global one
         (export_to_autoround/export.py:303-318): full layer name -> the differing fields."""
         out = {}
         if not self.layer_config:
             return out
         base = self.scheme.to_dict()
-        for bi, block in enumerate(blocks):
-            self.quantizer.block_prefix = f"{prefix}.{bi}"
-            for n, m in block.named_modules():
-                if type(m) is nn.Linear or isinstance(m, export.QuantLinear):
-                    sc = self.quantizer.scheme_for(n, m)
-                    if sc is None:
-                        continue
-                    diff = {k: v for k, v in sc.to_dict().items() if base.get(k) != v}
-                    if diff:
-                        out[f"{prefix}.{bi}.{n}"] = diff
-        self.quantizer.block_prefix = None
+        for _, _, full, sc in self._block_layers(lambda m: type(m) is nn.Linear or isinstance(m, export.QuantLinear)):
+            if sc is None:
+                continue
+            diff = {k: v for k, v in sc.to_dict().items() if base.get(k) != v}
+            if diff:
+                out[full] = diff
         return out
 
     def quantize_and_save(self, output_dir: str = "tmp_autoround", format: Optional[str] = None, inplace: bool = True):

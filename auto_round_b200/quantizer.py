@@ -70,10 +70,10 @@ def lr_schedule_table(iters: int, lr: float, minmax_lr: float) -> np.ndarray:
 
 class TuneArena:
     """Flat storage for every tunable of one block: fp32 [ V_0 | V_1 | ... | scales ... ] (+ the best snapshot) and the bf16
-    weight gradients `gq` [ dWq_0 | dWq_1 | ... ] written by the grad-w GEMMs.  `legacy_grads` adds the fp32/bf16 pre-sign
-    gradient buffers of the micro-batch path (fused grad-w epilogue -> ar_signsgd_step)."""
+    weight gradients `gq` [ dWq_0 | dWq_1 | ... ] written by the grad-w GEMMs.  `with_grads` adds the fp32 pre-sign
+    gradient buffers of the micro-batch path (lm_head: fused grad-w epilogue -> ar_signsgd_step)."""
 
-    def __init__(self, specs: dict, device, grad_dtype=None):
+    def __init__(self, specs: dict, device, with_grads: bool = False):
         off = 0
         self.views = {}
         for name, spec in specs.items():
@@ -98,8 +98,8 @@ class TuneArena:
             goff += (spec.n * spec.k + 7) // 8 * 8    # 16-byte aligned segments (TMA store target)
         self.gq = torch.zeros(goff, dtype=torch.bfloat16, device=device)
         self.grads_v = self.grads_s = None
-        if grad_dtype is not None:
-            self.grads_v = torch.zeros(self.clamp_begin, dtype=grad_dtype, device=device)
+        if with_grads:
+            self.grads_v = torch.zeros(self.clamp_begin, dtype=torch.float32, device=device)
             self.grads_s = torch.zeros(off - self.clamp_begin, dtype=torch.float32, device=device)
 
     def layer_views(self, name: str) -> dict:
@@ -193,6 +193,20 @@ def default_layer_filter(name: str, module: nn.Module) -> bool:
     return type(module) is nn.Linear
 
 
+def valid_token_masks(input_ids, device, stacked: bool = False):
+    """Per-sample masks of the tokens that count in the loss (label id != -100, base.py:257-280), or None when every
+    token counts.  `input_ids`: list of [1, S] label ids (or None).  Returns a list of [S] bool tensors on `device`, or
+    with `stacked` one contiguous uint8 [n, S] tensor."""
+    if input_ids is None:
+        return None
+    masks = [(ids != -100).reshape(-1) for ids in input_ids]
+    if all(bool(m.all()) for m in masks):
+        return None
+    if stacked:
+        return torch.stack(masks).to(device=device, dtype=torch.uint8).contiguous()
+    return [m.to(device) for m in masks]
+
+
 def _causal_equivalent(masks, token_masks) -> bool:
     """True if every cached attention mask is plain causal except, at most, entries in the LAST query row whose
     token is excluded from the loss.  The reference builds exactly that mask for tensor datasets (last key masked,
@@ -240,7 +254,7 @@ class SignRoundQuantizer:
                  enable_quanted_input: bool = True, not_use_best_mse: bool = False, amp_dtype=torch.bfloat16,
                  layer_config: Optional[dict] = None, layer_filter=default_layer_filter,
                  dp: Optional[DataParallel] = None, gradient_accumulate_steps: int = 1, use_cuda_graph: bool = True,
-                 fuse_block_ops: bool = True, grad_dtype=None, enable_alg_ext: bool = False):
+                 fuse_block_ops: bool = True, enable_alg_ext: bool = False):
         self.scheme = scheme
         # sign_roundv2 (SignRoundV2Quantizer.prepare_run, sign_roundv2/quantizer.py:330-357): symmetric int / mx / nv layers
         # get a searched init scale with max_scale in [0, 2]; bits < 4 additionally switches to the outlier-suppressed loss
@@ -259,7 +273,6 @@ class SignRoundQuantizer:
         self.dp = dp or DataParallel()
         self.use_cuda_graph = use_cuda_graph
         self.fuse_block_ops = fuse_block_ops
-        self.grad_dtype = grad_dtype        # kept for API compatibility: the weight gradient is bf16 (autograd of F.linear)
         self.gradient_accumulate_steps = max(1, int(gradient_accumulate_steps or 1))
         self.last_result: Optional[TuneResult] = None
         self.last_arena = None
@@ -271,6 +284,24 @@ class SignRoundQuantizer:
         if self.iters >= 1000 and bits <= 3:
             return 2.0 / self.iters
         return 1.0 / max(self.iters, 1)
+
+    def _lr_table(self, bits: int, device) -> torch.Tensor:
+        """Flat device copy of lr_schedule_table for this run: (rounding lr, minmax lr) of every iteration."""
+        lr0 = self.compute_lr(bits)
+        mm_lr0 = float(self.minmax_lr) if self.minmax_lr is not None else lr0
+        if not self.enable_minmax_tuning:
+            mm_lr0 = 0.0
+        return torch.from_numpy(lr_schedule_table(self.iters, lr0, mm_lr0)).to(device).reshape(-1)
+
+    def _read_losses(self, res: TuneResult, state: torch.Tensor, hist: torch.Tensor):
+        """Device loss state of a finished tuning loop -> `res` (the only host sync of the loop).  With not_use_best_mse
+        the last iteration is the one applied."""
+        st = state.cpu().tolist()
+        res.losses = hist.cpu().tolist()[:self.iters]
+        res.best_loss, res.best_iter = st[0], int(st[2])
+        res.init_loss = res.losses[0]
+        if self.not_use_best_mse:
+            res.best_iter, res.best_loss = self.iters - 1, res.losses[-1]
 
     def scheme_for(self, name: str, module: nn.Module) -> Optional[QuantizationScheme]:
         """Per-layer override: `layer_config` keys are FULL module names as in the reference
@@ -412,11 +443,7 @@ class SignRoundQuantizer:
         nsamples = x_all.shape[0]
         seq, hidden = x_all.shape[1], x_all.shape[-1]
 
-        token_masks = None
-        if input_ids is not None:
-            masks = [(ids != -100).reshape(-1) for ids in input_ids]
-            if not all(bool(m.all()) for m in masks):                     # base.py:257-280
-                token_masks = torch.stack(masks).to(device=device, dtype=torch.uint8).contiguous()
+        token_masks = valid_token_masks(input_ids, device, stacked=True)
         valid_per_sample = None if token_masks is None else token_masks.sum(dim=1).cpu().tolist()
 
         wrapped, arena = self.wrapper_block(block, nv_global_scales, kwargs.get("imatrices"))
@@ -447,12 +474,7 @@ class SignRoundQuantizer:
         if lbs == 0 or any(len(m) != lbs for it_m in micro for m in it_m):
             raise RuntimeError(f"micro-batches of {mbs} samples (global batch {gbs}) cannot be sharded evenly over {dp.world} ranks")
         idx_dev = torch.tensor(micro, dtype=torch.int32, device=device).reshape(iters, accum * lbs)
-        bits_all = {wl.scheme.bits for wl in wrapped.values()}
-        lr0 = self.compute_lr(min(bits_all))
-        mm_lr0 = float(self.minmax_lr) if self.minmax_lr is not None else lr0
-        if not self.enable_minmax_tuning:
-            mm_lr0 = 0.0
-        lr_tab = torch.from_numpy(lr_schedule_table(iters, lr0, mm_lr0)).to(device).reshape(-1)
+        lr_tab = self._lr_table(min(wl.scheme.bits for wl in wrapped.values()), device)
 
         loss_sum = torch.zeros(1, dtype=torch.float64, device=device)
         state = torch.zeros(4, dtype=torch.float64, device=device)
@@ -680,12 +702,7 @@ class SignRoundQuantizer:
                     per = kp if key == "value" else gpr
                     dp.all_gather_(flat, flat[r0 * per:r1 * per])
 
-        st = state.cpu().tolist()                                   # the only host sync of the block
-        res.losses = hist.cpu().tolist()
-        res.best_loss, res.best_iter = st[0], int(st[2])
-        res.init_loss = res.losses[0]
-        if self.not_use_best_mse:
-            res.best_iter, res.best_loss = iters - 1, res.losses[-1]
+        self._read_losses(res, state, hist)
         with torch.no_grad():
             self.unwrapper_block(block, wrapped, arena)
         for m in moe_mods:
@@ -712,7 +729,7 @@ class SignRoundQuantizer:
         sc = self.scheme_for(name, layer)
         n, k = layer.weight.shape
         spec = ops.make_spec(sc.qdq_name, sc.bits, sc.group_size, n, k, 1e-5, 1.0)
-        arena = TuneArena({name: spec}, device, torch.float32)
+        arena = TuneArena({name: spec}, device, with_grads=True)
         gs = kwargs.get("nv_global_scale")
         wl = WrapperLinear(layer, sc, spec, arena.layer_views(name), gs)
         nsamples = len(fp_inputs)
@@ -720,11 +737,7 @@ class SignRoundQuantizer:
         seq = fp_all.shape[1]
         fp_all = fp_all.reshape(nsamples, seq, k).contiguous()
         q_all = None if q_inputs is None else self._stack(q_inputs, device).to(torch.bfloat16).reshape(nsamples, seq, k).contiguous()
-        token_masks = None
-        if input_ids is not None:
-            masks = [(ids != -100).reshape(-1) for ids in input_ids]
-            if not all(bool(m.all()) for m in masks):
-                token_masks = torch.stack(masks).to(device=device, dtype=torch.uint8).contiguous()
+        token_masks = valid_token_masks(input_ids, device, stacked=True)
         iters = self.iters
         gbs = min(nsamples, self.batch_size)                       # gradient_accumulate_steps = batch_size (:660-662)
         if self.batch_size != 1:
@@ -740,11 +753,7 @@ class SignRoundQuantizer:
         batches = [list(sampler.next_batch()) for _ in range(iters)]
         res = TuneResult(quantized_layers=[name], batches=batches)
         self.last_result = res
-        lr0 = self.compute_lr(sc.bits)
-        mm_lr0 = float(self.minmax_lr) if self.minmax_lr is not None else lr0
-        if not self.enable_minmax_tuning:
-            mm_lr0 = 0.0
-        lr_tab = torch.from_numpy(lr_schedule_table(iters, lr0, mm_lr0)).to(device).reshape(-1)
+        lr_tab = self._lr_table(sc.bits, device)
         loss_sum = torch.zeros(1, dtype=torch.float64, device=device)
         state = torch.zeros(4, dtype=torch.float64, device=device)
         flag = torch.zeros(1, dtype=torch.int32, device=device)
@@ -773,11 +782,7 @@ class SignRoundQuantizer:
             ops.signsgd_step(arena.params, arena.grads_v, arena.best, flag, lr_tab, it, arena.clamp_begin, 1.0,
                              g_scales=arena.grads_s)
         if iters > 0:
-            st = state.cpu().tolist()
-            res.losses = hist.cpu().tolist()[:iters]
-            res.best_loss, res.best_iter, res.init_loss = st[0], int(st[2]), res.losses[0]
-            if self.not_use_best_mse:
-                res.best_iter, res.best_loss = iters - 1, res.losses[-1]
+            self._read_losses(res, state, hist)
             with torch.no_grad():
                 lin = wl.unwrapper(arena.best_views(name))
         else:

@@ -1,6 +1,5 @@
 """bf16 pre-sign gradient path used under data parallelism: the fused dW epilogue can emit dV in bf16 (half the NVLink
-exchange); the update only uses the sign.  Checks: bf16 dV == bf16-rounded fp32 dV, identical sign-SGD step, and a
-whole tuned block with grad_dtype=bf16 lands within the same tolerance band as fp32."""
+exchange); the update only uses the sign.  Checks: bf16 dV == bf16-rounded fp32 dV and an identical sign-SGD step."""
 import pytest
 import torch
 
