@@ -3,18 +3,22 @@
 //   D[M,N] = A[M,K] · B[N,K]ᵀ ,  fp32 accumulate in registers, operands staged by TMA into 128B-swizzled smem.
 //
 // One persistent CTA per SM (132 on an H100 SXM), warp-specialised:
-//   warps 0..7  two consumer warpgroups: warpgroup w issues wgmma.m64n128k16 for rows [64w, 64w+64) of the 128 x 128
-//               tile, then both run the epilogue from an fp32 staging tile in smem
+//   warps 0..7  two consumer warpgroups: warpgroup w issues wgmma.m64n{BN}k16 for rows [64w, 64w+64) of the 128 x BN
+//               tile, then runs the epilogue of its own rows
 //   warp 8      TMA producer   (one elected lane; mbarrier full/empty ring; keeps loading the next tile's stages while
 //                               the consumers run the epilogue of the current one)
+// Tile width BN per epilogue: EPI_STORE uses 128 x 256 tiles (m64n256k16 reads 17 % fewer smem bytes per FLOP than
+// m64n128k16, and each staged A slab feeds twice the output columns); EPI_DW keeps 128 x 128 tiles because its fp32
+// staging tile would not fit beside a 128 x 256 operand ring.
 // Each operand may be K-major (reduction dim contiguous) or MN-major (row dim contiguous), which covers the
 // three GEMMs of a linear without any transposed copies (wgmma's transpose bits read MN-major bf16 directly):
 //   forward   Y  = X  · Wqᵀ      A = X  [T,K]  K-major      B = Wq [N,K]  K-major
 //   grad-in   dX = dY · Wq       A = dY [T,N]  K-major      B = Wq [N,K]  as [K_out, N_red]: MN-major
 //   grad-w    dW = dYᵀ· X        A = dY [T,N]  as [N_out, T_red]: MN-major   B = X [T,K] as [K_out, T_red]: MN-major
 // Epilogues:
-//   EPI_STORE  fp32 -> (+bias) -> bf16 -> global (16-byte stores, clipped to the problem)
-//   EPI_DW     fp32 dWq tile -> fake-quant backward in registers -> dV (fp32), d min/max_scale per group; the
+//   EPI_STORE  fp32 registers -> (+bias) -> bf16 -> global, straight from each warpgroup's accumulators (a quad
+//              transpose gives 16-byte stores; clipped to the problem); no smem staging and no consumer barrier
+//   EPI_DW     fp32 dWq tile -> smem staging tile -> fake-quant backward in registers -> dV (fp32), d min/max_scale per group; the
 //              dWq matrix itself is never written (auto_round: autograd through wrapper.py:273-290)
 // FLOPs per launch = 2*M*N*K; roofline = dense bf16 tensor peak (MEASURED_PEAKS.json: bf16_tflops).
 #include <cuda.h>
@@ -29,7 +33,8 @@
 namespace ar {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 128;
+constexpr int kStoreBN = 256;         // tile width of the EPI_STORE launches
+constexpr int kDwBN = 128;            // tile width of the EPI_DW launches
 constexpr int BLOCK_K = 64;           // 64 bf16 = 128 B = one swizzle atom row
 constexpr int WGMMA_K = 16;
 constexpr int kStages = 4;
@@ -136,6 +141,49 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a
       : "memory");
 }
 
+// D(64 x 256, fp32, registers) += A(64 x 16) · B(256 x 16)ᵀ; same fragment layout as m64n128k16 with j in [0, 32).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, "
+      "%128, %129, 1, 1, 1, %130, %131;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+        "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+        "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]),
+        "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+        "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+        "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]),
+        "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]),
+        "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]),
+        "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]),
+        "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]),
+        "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t desc_a, uint64_t desc_b) {
+  if constexpr (BN == 256) wgmma_m64n256k16<TA, TB>(d, desc_a, desc_b);
+  else wgmma_m64n128k16<TA, TB>(d, desc_a, desc_b);
+}
+
 // ---------------------------------------------------------------------------------------- kernel params
 struct DwParams {                 // EPI_DW: fake-quant backward inputs/outputs
   const uint16_t* w;              // bf16 [N,K]
@@ -193,20 +241,23 @@ struct GemmParams {
   DwParams dw;
 };
 
-// Staging tile of the epilogue: fp32 [BLOCK_M][kStageLd]; the pad of 8 floats makes the float2 fragment stores of a
-// half-warp (4 rows x 4 column pairs) hit 32 distinct banks.
-constexpr int kStageLd = BLOCK_N + 8;
+// Staging tile of the EPI_DW epilogue: fp32 [BLOCK_M][kStageLd]; the pad of 8 floats makes the float2 fragment stores
+// of a half-warp (4 rows x 4 column pairs) hit 32 distinct banks.  EPI_STORE has no staging tile.
+constexpr int kStageLd = kDwBN + 8;
+template <int BN, bool STAGED>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;       // 16 KB
-  static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;       // 16 KB
+  static constexpr int kBBytes = BN * BLOCK_K * 2;            // 16 KB (BN 128) or 32 KB (BN 256)
   static constexpr int kAOff = 0;
   static constexpr int kBOff = kStages * kABytes;
   static constexpr int kCOff = kBOff + kStages * kBBytes;
-  static constexpr int kCBytes = BLOCK_M * kStageLd * 4;      // 68 KB
+  static constexpr int kCBytes = STAGED ? BLOCK_M * kStageLd * 4 : 0;   // 68 KB
   static constexpr int kBarOff = kCOff + kCBytes;
   static constexpr int kTotal = kBarOff + 512 + 1024;         // + slack to align the base to 1024 B (SWIZZLE_128B atoms)
+  static_assert(kTotal <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
 };
-static_assert(SmemLayout::kTotal <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
+using StoreSmem = SmemLayout<kStoreBN, false>;                // 4 x 48 KB ring = 192 KB
+using DwSmem = SmemLayout<kDwBN, true>;                       // 4 x 32 KB ring + 68 KB staging = 196 KB
 constexpr int kSchedSlots = 8;
 
 // tile order: groups of 8 M-tiles sweep all N-tiles, so the concurrent CTAs share A/B tiles in L2
@@ -221,7 +272,7 @@ __device__ __forceinline__ void tile_coords(int t, int m_tiles, int n_tiles, int
   nt = in / gm;
 }
 
-template <bool B_MN>
+template <int BN, bool B_MN>
 __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int m_tiles, int num_kb_static) {
   TileInfo ti;
   int mt, nt;
@@ -231,7 +282,7 @@ __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int
     tile_coords(t - ae * per, p.m_tiles, p.n_tiles, mt, nt);
     const int e = p.grp.table[3 * ae], koff = p.grp.table[3 * ae + 1], klen = p.grp.table[3 * ae + 2];
     ti.m0 = mt * BLOCK_M;
-    ti.n0 = nt * BLOCK_N;
+    ti.n0 = nt * BN;
     ti.d_m0 = e * p.grp.d_group_rows + ti.m0;
     ti.d_n0 = ti.n0;
     ti.a_koff = koff;
@@ -240,7 +291,7 @@ __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int
     return ti;
   }
   tile_coords(t, m_tiles, p.n_tiles, mt, nt);
-  ti.n0 = nt * BLOCK_N;
+  ti.n0 = nt * BN;
   ti.d_n0 = ti.n0;
   ti.a_koff = 0;
   ti.b_koff = 0;
@@ -385,31 +436,54 @@ __device__ __forceinline__ void epilogue_dw(const GemmParams& p, const float* ac
   }
 }
 
-// bf16 store epilogue: thread handles 8 consecutive columns of one row per step (a warp writes two 256-byte row pieces)
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float* stage, int m0, int n0, int ctid) {
-  constexpr int kChunks = BLOCK_N / 8;
-#pragma unroll 1
-  for (int u = ctid; u < BLOCK_M * kChunks; u += kConsumerThreads) {
-    const int r = u / kChunks, c = (u % kChunks) * 8;
-    const int row = m0 + r, col = n0 + c;
-    if (row >= p.d_rows || col >= p.n) continue;
-    const float4 q0 = *reinterpret_cast<const float4*>(stage + r * kStageLd + c);
-    const float4 q1 = *reinterpret_cast<const float4*>(stage + r * kStageLd + c + 4);
-    float x[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-    if (p.bias) {
-      // F.linear under autocast: bf16 GEMM result (+bias in fp32 inside the fused epilogue)
+// bf16 store epilogue straight from one warpgroup's accumulators.  Thread (warp w of the warpgroup, lane l) holds
+// D[16w + l/4 + 8h][8j + 2(l%4) + e] in acc[4j + 2h + e]; `row0` is the output row of h = 0.  After the bias and the
+// rounding to bf16 pairs, a 4 x 4 transpose inside each quad (two shfl.xor rounds) hands lane q of the quad the 8
+// consecutive columns 8(4b + q) .. +7 of its row, so each 16-byte store of a warp writes 8 rows x 64 contiguous bytes.
+template <int BN>
+__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float (&acc)[BN / 2], int row0, int n0, int lane) {
+  const int q = lane & 3;
+  const bool odd = (q & 1) != 0, hi = (q & 2) != 0;
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        if (col + i < p.n) x[i] += bf16_bits_to_f32(p.bias[col + i]);
+  for (int b = 0; b < BN / 32; ++b) {
+    uint32_t v[2][4];                                      // [h][s]: bf16 pair of columns 8(4b + s) + 2q, +1
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int j = 4 * b + s;
+      float x[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+      if (p.bias) {
+        // F.linear under autocast: bf16 GEMM result (+bias in fp32 inside the fused epilogue)
+        const int col = n0 + 8 * j + 2 * q;
+        const float b0 = col < p.n ? bf16_bits_to_f32(p.bias[col]) : 0.f;
+        const float b1 = col + 1 < p.n ? bf16_bits_to_f32(p.bias[col + 1]) : 0.f;
+        if (col < p.n) { x[0] += b0; x[2] += b0; }
+        if (col + 1 < p.n) { x[1] += b1; x[3] += b1; }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        v[h][s] = (uint32_t)f32_to_bf16_bits(x[2 * h]) | ((uint32_t)f32_to_bf16_bits(x[2 * h + 1]) << 16);
     }
-    uint16_t* o = p.d + (int64_t)row * p.ldd + col;
-    if (col + 8 <= p.n) {
-      uint32_t pk[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) pk[i] = (uint32_t)f32_to_bf16_bits(x[2 * i]) | ((uint32_t)f32_to_bf16_bits(x[2 * i + 1]) << 16);
-      *reinterpret_cast<U4*>(o) = U4{pk[0], pk[1], pk[2], pk[3]};
-    } else {
-      for (int i = 0; col + i < p.n; ++i) o[i] = f32_to_bf16_bits(x[i]);
+    for (int h = 0; h < 2; ++h) {
+      uint32_t* u = v[h];
+      // round 1 (lanes q, q^1): swap the slots whose bit 0 differs from q's; round 2 (q, q^2): the same for bit 1.
+      // Afterwards slot s of lane q holds the pair lane s had for j = 4b + q.
+      uint32_t t0 = __shfl_xor_sync(0xffffffffu, odd ? u[0] : u[1], 1);
+      uint32_t t1 = __shfl_xor_sync(0xffffffffu, odd ? u[2] : u[3], 1);
+      if (odd) { u[0] = t0; u[2] = t1; } else { u[1] = t0; u[3] = t1; }
+      t0 = __shfl_xor_sync(0xffffffffu, hi ? u[0] : u[2], 2);
+      t1 = __shfl_xor_sync(0xffffffffu, hi ? u[1] : u[3], 2);
+      if (hi) { u[0] = t0; u[1] = t1; } else { u[2] = t0; u[3] = t1; }
+      const int row = row0 + 8 * h, col = n0 + 8 * (4 * b + q);
+      if (row >= p.d_rows || col >= p.n) continue;
+      uint16_t* o = p.d + (int64_t)row * p.ldd + col;
+      if (col + 8 <= p.n) {
+        *reinterpret_cast<U4*>(o) = U4{u[0], u[1], u[2], u[3]};
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)                        // unrolled: constant register indices
+          if (col + i < p.n) o[i] = (uint16_t)(u[i >> 1] >> (16 * (i & 1)));
+      }
     }
   }
 }
@@ -421,10 +495,11 @@ __device__ __forceinline__ void epilogue_store(const GemmParams& p, const float*
 // when NCCL kernels of the data-parallel exchange hold a few SMs while a GEMM launches (they cannot co-reside with a 200 KB
 // CTA).  With tickets, late CTAs simply find the queue empty.  Ticket order = rasterised tile order, so concurrently
 // running CTAs still work on neighbouring tiles (L2 reuse).  The CTA that draws the last terminal ticket resets the counter.
-template <bool A_MN, bool B_MN, int EPI, class Ctx, int G, bool IS_FP4>
+template <int BN, bool A_MN, bool B_MN, int EPI, class Ctx, int G, bool IS_FP4>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
-  using L = SmemLayout;
+  static_assert(EPI == EPI_STORE || BN == kDwBN, "the EPI_DW staging tile is 128 columns wide");
+  using L = SmemLayout<BN, EPI == EPI_DW>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -433,7 +508,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
   uint64_t* sfull = bars + 2 * kStages;           // [kSchedSlots] ticket published
   uint64_t* sempty = sfull + kSchedSlots;         // [kSchedSlots] ticket read by all eight consumer warps
   volatile int32_t* stile = reinterpret_cast<volatile int32_t*>(sempty + kSchedSlots);   // [kSchedSlots]
-  float* stage = reinterpret_cast<float*>(smem + L::kCOff);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -465,7 +539,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         mbar_arrive(&sfull[slot]);
         if (t >= num_tiles) break;
         t_next = (int)atomicAdd(p.tile_ctr, 1u);           // next ticket: in flight while this tile's loads are issued
-        const TileInfo ti = resolve_tile<B_MN>(p, t, m_tiles_dyn, num_kb);
+        const TileInfo ti = resolve_tile<BN, B_MN>(p, t, m_tiles_dyn, num_kb);
         for (int kb = 0; kb < ti.num_kb; ++kb, ++it) {
           const uint32_t s = it % kStages, sph = (it / kStages) & 1u;
           mbar_wait(&empty[s], sph ^ 1u);
@@ -481,10 +555,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
               tma_load_2d(sa + i * (64 * BLOCK_K * 2), &map_a, &full[s], ti.m0 + i * 64, ti.a_koff + k0);
           }
           if (!B_MN) {
-            tma_load_2d(sb, &map_b, &full[s], ti.b_koff + k0, ti.n0);                 // box {64 k, 128 n}
+            tma_load_2d(sb, &map_b, &full[s], ti.b_koff + k0, ti.n0);                 // box {64 k, BN n}
           } else {
 #pragma unroll
-            for (int i = 0; i < BLOCK_N / 64; ++i)
+            for (int i = 0; i < BN / 64; ++i)
               tma_load_2d(sb + i * (64 * BLOCK_K * 2), &map_b, &full[s], ti.n0 + i * 64, ti.b_koff + k0);
           }
         }
@@ -509,11 +583,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       __syncwarp();
       if (lane == 0) mbar_arrive(&sempty[slot]);
       if (t >= num_tiles) break;
-      const TileInfo ti = resolve_tile<B_MN>(p, t, m_tiles_dyn, num_kb);
+      const TileInfo ti = resolve_tile<BN, B_MN>(p, t, m_tiles_dyn, num_kb);
 
-      float acc[64];
+      float acc[BN / 2];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       uint32_t prev = 0;
       for (int kb = 0; kb < ti.num_kb; ++kb, ++it) {
         const uint32_t s = it % kStages, sph = (it / kStages) & 1u;
@@ -523,8 +597,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
-          wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, make_smem_desc(sa + k * a_kstep, a_lbo, 1024),
-                                                        make_smem_desc(sb + k * b_kstep, b_lbo, 1024));
+          wgmma_tile_k16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, make_smem_desc(sa + k * a_kstep, a_lbo, 1024),
+                                                         make_smem_desc(sb + k * b_kstep, b_lbo, 1024));
         wgmma_commit();
         wgmma_wait<1>();                                   // the previous stage's MMAs have retired: hand it back
         if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
@@ -533,24 +607,26 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       wgmma_wait<0>();
       if (ti.num_kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
 
-      consumer_bar_sync();                                 // the previous tile's epilogue is done reading the staging tile
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = 8 * j + 2 * (lane & 3);
-        const int r0 = wg * 64 + wrow;
-        *reinterpret_cast<float2*>(stage + r0 * kStageLd + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(stage + (r0 + 8) * kStageLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      consumer_bar_sync();
       if constexpr (EPI == EPI_DW) {
+        float* stage = reinterpret_cast<float*>(smem + L::kCOff);
+        consumer_bar_sync();                               // the previous tile's epilogue is done reading the staging tile
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          const int r0 = wg * 64 + wrow;
+          *reinterpret_cast<float2*>(stage + r0 * kStageLd + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(stage + (r0 + 8) * kStageLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        consumer_bar_sync();
         constexpr int SPAN = (G > 64) ? G : 64;            // whole groups per thread
-        constexpr int kUnits = BLOCK_M * (BLOCK_N / SPAN);
+        constexpr int kUnits = BLOCK_M * (BN / SPAN);
         if (ctid < kUnits) {
           const int r = ctid % BLOCK_M, c = (ctid / BLOCK_M) * SPAN;
           epilogue_dw<Ctx, G, IS_FP4, SPAN>(p, stage + r * kStageLd + c, ti.d_m0 + r, ti.d_n0 + c);
         }
       } else {
-        epilogue_store(p, stage, ti.d_m0, ti.d_n0, ctid);
+        // each warpgroup stores its own 64 rows and moves on to the next ticket: no consumer-wide barrier
+        epilogue_store<BN>(p, acc, ti.d_m0 + wg * 64 + wrow, ti.d_n0, lane);
       }
     }
   }
@@ -628,8 +704,9 @@ static unsigned int* next_tile_counter() {
 template <bool A_MN, bool B_MN, int EPI, class Ctx, int G, bool IS_FP4>
 static int launch(const void* a, const void* b, void* d, int m, int n, int k, int64_t lda, int64_t ldb, int64_t ldd,
                   const GemmParams& base, cudaStream_t st) {
-  using L = SmemLayout;
-  auto kern = gemm_kernel<A_MN, B_MN, EPI, Ctx, G, IS_FP4>;
+  constexpr int BN = (EPI == EPI_STORE) ? kStoreBN : kDwBN;
+  using L = SmemLayout<BN, EPI == EPI_DW>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, Ctx, G, IS_FP4>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
@@ -644,7 +721,7 @@ static int launch(const void* a, const void* b, void* d, int m, int n, int k, in
   if (rc) return rc;
   const uint64_t b_rows = base.b_rows_map > 0 ? (uint64_t)base.b_rows_map : (uint64_t)n;
   const uint64_t b_k = base.b_k_map > 0 ? (uint64_t)base.b_k_map : (uint64_t)k;
-  if (!B_MN) rc = make_map(&mb, b, b_k, b_rows, (uint64_t)ldb, 64, BLOCK_N);
+  if (!B_MN) rc = make_map(&mb, b, b_k, b_rows, (uint64_t)ldb, 64, BN);
   else rc = make_map(&mb, b, b_rows, b_k, (uint64_t)ldb, 64, BLOCK_K);
   if (rc) return rc;
   GemmParams p = base;
@@ -660,7 +737,7 @@ static int launch(const void* a, const void* b, void* d, int m, int n, int k, in
   p.tile_ctr = next_tile_counter();
   AR_REQUIRE(p.tile_ctr != nullptr, AR_E_DRIVER, "tile counter symbol not available on this device");
   p.m_tiles = (m + BLOCK_M - 1) / BLOCK_M;
-  p.n_tiles = (n + BLOCK_N - 1) / BLOCK_N;
+  p.n_tiles = (n + BN - 1) / BN;
   const int tiles = base.max_tiles > 0 ? base.max_tiles : p.m_tiles * p.n_tiles;
   const int ctas = tiles < sm_count() ? tiles : sm_count();
   kern<<<(unsigned)ctas, kNumThreads, L::kTotal, st>>>(ma, mb, p);
@@ -699,7 +776,7 @@ extern "C" int ar_gemm_bf16_grouped(const void* a, const void* b, void* d, int m
   p.grp.table = table;
   p.grp.num = num;
   cudaStream_t st = (cudaStream_t)stream;
-  const int n_tiles = (n + BLOCK_N - 1) / BLOCK_N;
+  const int n_tiles = (n + kStoreBN - 1) / kStoreBN;     // both grouped modes launch EPI_STORE instantiations
   if (mode == GROUP_M) {
     // D[rows, n] = A[rows, k] * B_e^T, e = expert of the row tile.  B stacked over experts: K-major [G * group_rows, k]
     // (forward: group_rows = n) or stored [G * group_rows, n] read MN-major with the reduction inside the expert's rows
