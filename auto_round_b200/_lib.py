@@ -57,6 +57,8 @@ SIGNATURES = {
     "ar_gather_rows": [_P, _P, _I, _L, _P, _P],
     "ar_pack_int": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P],
     "ar_unpack_int": [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P],
+    "ar_pack_awq": [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P],
+    "ar_unpack_awq": [_P, _P, _P, _I, _I, _I, _P, _P, _P],
     "ar_pack_fp4_nv": [_P, _P, _P, _I, _I, _P, _P, _P],
     "ar_pack_fp4_mx": [_P, _P, _I, _I, _P, _P, _P],
     "ar_unpack_fp4": [_P, _I, _I, _P, _P],

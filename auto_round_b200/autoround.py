@@ -7,7 +7,8 @@
     model, layer_config = ar.quantize()
     ar.quantize_and_save("out_dir", format="auto_round")
 
-Out of scope (rejected loudly, never silently emulated): activation quantisation, GGUF / AWQ / MLX formats,
+Checkpoint formats: "auto_round" (default), "auto_gptq", "auto_awq" (export.resolve_format).
+Out of scope (rejected loudly, never silently emulated): activation quantisation, GGUF / MLX / llm-compressor formats,
 AutoScheme, MLLM / diffusion calibration, torch.compile, CPU execution.
 """
 from __future__ import annotations
@@ -249,6 +250,7 @@ class AutoRound:
         self.timings = {}
         self._pack_on_the_fly = False
         self._packed = False
+        self._fmt = None                        # export.ResolvedFormat the layers are (to be) packed in
         self._lm_head_extra = None              # {name: extra_config entry} of layers quantized outside the blocks
 
     # -------------------------------------------------------------------------------------------
@@ -449,6 +451,8 @@ class AutoRound:
         model = self.model
         prefix, blocks = find_blocks(model)
         self.block_prefix, self._blocks = prefix, blocks
+        if self._pack_on_the_fly and self._fmt is None:
+            self._fmt = self._resolve_format("auto_round")
         mode = "tune" if self.iters > 0 else self._rtn_mode()
         tune = mode == "tune"
         fp_inputs = others = ids_cache = token_masks = None
@@ -548,7 +552,7 @@ class AutoRound:
             if self._pack_on_the_fly:                                     # immediate_pack (orchestrator.py:327-337)
                 for n in done:
                     export.pack_layer(n, block, quantizer.scheme_for(n, block.get_submodule(n)), self.device,
-                                      out_device=self.device)
+                                      out_device=self.device, fmt=self._fmt)
             if tune:
                 ev[4].record()
             self._hook(bi, "d2h0")
@@ -646,7 +650,7 @@ class AutoRound:
         self.block_results.append({"block": name, "init_loss": res.init_loss, "best_loss": res.best_loss,
                                    "best_iter": res.best_iter, "losses": res.losses})
         if self._pack_on_the_fly:
-            export.pack_layer(name, self.model, sc, self.device, out_device=self.device)
+            export.pack_layer(name, self.model, sc, self.device, out_device=self.device, fmt=self._fmt)
         self._lm_head_extra = {name: export.extra_config_entry(sc)}
         norm.to("cpu")
         self.model.get_submodule(name).to("cpu")
@@ -662,6 +666,8 @@ class AutoRound:
                        + resume_mod.layer_config_fingerprint(self.layer_config)
                        + f"|iters={self.iters}|bs={self.batch_size}|seed={self.seed}|alg_ext={getattr(self, 'enable_alg_ext', False)}"
                        + f"|pack={self._pack_on_the_fly}|{sorted(self.sign_kw.items())}")
+        if self._pack_on_the_fly and self._fmt is not None and self._fmt.is_new_layout:
+            scheme_desc += f"|layout={self._fmt.writer}/{self._fmt.layout}"      # a resumed run cannot mix layouts
         sig = resume_mod.compute_run_signature(model_id, scheme_desc, resume_mod.dataset_fingerprint(self.dataset), self.nsamples,
                                                self.seqlen, names)
         st = resume_mod.ResumeState(os.path.join(rd, "group_0"), sig, names)
@@ -685,34 +691,95 @@ class AutoRound:
             return "calibrated_opt"
         return "calibrated_opt" if name == "nv_fp4" else "zero_shot_opt"
 
+    def _resolve_format(self, format: Optional[str]):
+        """export.resolve_format for this run: host-only checks of `format` against the scheme, `layer_config` and the
+        shapes of the linears that will be quantised (the blocks', and lm_head with quant_lm_head)."""
+        base = self.scheme.to_dict()
+        layers = []
+        try:
+            prefix, blocks = find_blocks(self.model)
+        except RuntimeError:
+            prefix, blocks = None, []
+        named = [(f"{prefix}.{bi}.{n}", n, m) for bi, blk in enumerate(blocks) for n, m in blk.named_modules()]
+        if self.quant_lm_head and isinstance(getattr(self.model, "lm_head", None), nn.Linear):
+            named.append(("lm_head", "lm_head", self.model.lm_head))
+        for full, rel, m in named:
+            if type(m) is not nn.Linear:
+                continue
+            cfg = self.layer_config.get(full, self.layer_config.get(rel))
+            sc = cfg if isinstance(cfg, QuantizationScheme) else QuantizationScheme.from_dict({**base, **(cfg or {})})
+            if sc.bits <= 8:
+                layers.append((full, m, sc))
+        return export.resolve_format(format, self.scheme, self.layer_config, layers)
+
     def save_quantized(self, output_dir: Optional[str] = None, format: str = "auto_round", inplace: bool = True):
-        if format not in ("auto_round", "auto_round:auto_gptq"):
-            raise NotImplementedError(f"format {format!r}: only the auto_round checkpoint format is in scope")
+        fmt = self._resolve_format(format) if not self._packed else self._resolve_format_packed(format)
         if not self.quantized:
             raise RuntimeError("call quantize() first")
         if not self._packed:
             for block, n, _, sc in self._block_layers(lambda m: type(m) is nn.Linear and hasattr(m, "scale")):
-                export.pack_layer(n, block, sc, self.device)
+                export.pack_layer(n, block, sc, self.device, fmt=fmt)
             for n in (self._lm_head_extra or {}):                           # layers tuned outside the blocks (lm_head)
                 m = self.model.get_submodule(n)
                 if type(m) is nn.Linear and hasattr(m, "scale"):
-                    export.pack_layer(n, self.model, self.quantizer.scheme_for(n, m), self.device)
-            self._packed = True
-        extra = dict(self._lm_head_extra or {})
-        extra.update(self._layer_config_overrides())
+                    export.pack_layer(n, self.model, self.quantizer.scheme_for(n, m), self.device, fmt=fmt)
+            self._packed, self._fmt = True, fmt
         tuning = dict(self.sign_kw)
         lr_used = self.quantizer.compute_lr(self.scheme.bits) if self.iters > 0 else None
         if lr_used is not None and "lr" not in tuning and lr_used != 1.0 / self.iters:
             tuning["lr"] = lr_used                    # the auto rule gave 2/iters: the reference serialises the resolved lr
             tuning.setdefault("minmax_lr", lr_used)
-        qcfg = export.build_quantization_config(self.scheme, self.block_prefix, extra or None, self.iters,
-                                                self.nsamples, self.seqlen, self.batch_size, tuning=tuning)
+        if fmt.writer == "auto_round":
+            extra = dict(self._lm_head_extra or {})
+            extra.update(self._layer_config_overrides())
+            qcfg = export.build_quantization_config(self.scheme, self.block_prefix, extra or None, self.iters,
+                                                    self.nsamples, self.seqlen, self.batch_size, tuning=tuning,
+                                                    packing_format=fmt.packing_format)
+        elif fmt.writer == "auto_awq":
+            qcfg = export.build_awq_config(self.scheme, self.block_prefix, self._unquantized_linears(), self.iters, tuning)
+        else:
+            qcfg = self._gptq_config(tuning)
         self.quantization_config = qcfg
         if output_dir is None:
             self.model.config.quantization_config = qcfg
             return self.model
-        export.save_quantized(self.model, output_dir, qcfg, self.tokenizer)
+        export.save_quantized(self.model, output_dir, qcfg, self.tokenizer, fp16=fmt.writer != "auto_round")
         return self.model
+
+    def _resolve_format_packed(self, format: Optional[str]):
+        """The layers are packed already (quantize_and_save, or an earlier save): `format` must resolve to that layout;
+        packed words are not re-packed into another one."""
+        fmt = self._resolve_format(format)
+        have = self._fmt if self._fmt is not None else self._resolve_format("auto_round")
+        if (fmt.writer == "auto_gptq") != (have.writer == "auto_gptq") or fmt.layout != have.layout:
+            raise RuntimeError(f"the model is already packed for {have.writer} ({have.layout} layout); format {format!r} "
+                               f"needs the {fmt.layout} layout of {fmt.writer}.  Choose the format before packing: "
+                               "quantize_and_save(format=...), or quantize() then save_quantized(format=...)")
+        return fmt
+
+    def _unquantized_linears(self) -> list:
+        """Full names of the nn.Linear layers the run left in 16 bit (`modules_to_not_convert` of the AWQ config,
+        export_to_awq/export.py:60-111)."""
+        return [n for n, m in self.model.named_modules() if type(m) is nn.Linear]
+
+    def _gptq_config(self, tuning: dict) -> dict:
+        """export_to_autogptq/export.py:232-310: per-layer overrides become `dynamic` rules, a quantised lm_head sets
+        `lm_head`, and when a block layer stays unquantised the block-relative names of the quantised ones are listed."""
+        base = self.scheme.to_dict()
+        overrides, quantized, all_quantized = {}, set(), True
+        both = lambda m: type(m) is nn.Linear or isinstance(m, export.QuantLinear)           # noqa: E731
+        for block, n, full, sc in self._block_layers(both):
+            if isinstance(block.get_submodule(n), export.QuantLinear):
+                quantized.add(n)
+            else:
+                all_quantized = False
+            if sc is not None and any(base.get(k) != v for k, v in sc.to_dict().items()):
+                overrides[full] = sc
+        for n in (self._lm_head_extra or {}):
+            overrides[n] = self.quantizer.scheme_for(n, self.model.get_submodule(n))
+        return export.build_gptq_config(self.scheme, overrides, bool(self._lm_head_extra),
+                                        None if all_quantized else [sorted(quantized)],
+                                        self.iters, tuning)
 
     def _layer_config_overrides(self) -> dict:
         """`extra_config` entries for block layers whose resolved scheme differs from the global one
@@ -731,6 +798,7 @@ class AutoRound:
 
     def quantize_and_save(self, output_dir: str = "tmp_autoround", format: Optional[str] = None, inplace: bool = True):
         fmt = format or "auto_round"
+        self._fmt = self._resolve_format(fmt)             # rejects an unsupported combination before any GPU work
         self._pack_on_the_fly = True
         model, _ = self.quantize()
         self.save_quantized(output_dir, fmt, inplace)

@@ -204,6 +204,96 @@ __global__ void unpack_int_kernel(const int32_t* __restrict__ qweight, const int
   }
 }
 
+// ---- AWQ "GEMM" layout, 4 bit (auto_round/export/export_to_awq/utils.py:197-273): the eight codes of output columns
+// 8j .. 8j+7 of one k go into word j of row k, column 8j+i at bit 4 * order[i].  The words run along N while the weight is
+// row-major in K, so a tile of 128 rows x 64 k is turned through shared memory: a thread loads 16 B (8 k of one row, a
+// warp covers 128 B of each of 4 rows), codes them against one scale / zero-point (a group is a multiple of 8 k) and
+// parks them as 8 bytes; then a thread gathers the 8 rows of one word column for those 8 k and writes 8 words, a warp
+// covering 64 B of each of 2 output rows per store.  Bytes per weight: 2 read + 0.5 written.
+__device__ __constant__ int kAwqShift[8] = {0, 16, 4, 20, 8, 24, 12, 28};            // 4 * [0, 4, 1, 5, 2, 6, 3, 7]
+constexpr int AWQ_TN = 128, AWQ_TK = 64;
+
+__global__ void __launch_bounds__(256) pack_awq_kernel(const uint16_t* __restrict__ wq, const __half* __restrict__ scale,
+                                                       const float* __restrict__ zp, float zp_const, int n, int k,
+                                                       int group_size, int32_t* __restrict__ qweight) {
+  __shared__ U2 tile[AWQ_TN][AWQ_TK / 8 + 1];         // [row][k chunk] -> 8 int8 codes
+  const int ngroups = k / group_size;
+  const int row0 = blockIdx.y * AWQ_TN, k0 = blockIdx.x * AWQ_TK;
+  for (int t = threadIdx.x; t < AWQ_TN * (AWQ_TK / 8); t += 256) {
+    const int r = t / (AWQ_TK / 8), c = t % (AWQ_TK / 8);
+    const int row = row0 + r, kk = k0 + c * 8;
+    uint32_t lo = 0, hi = 0;
+    if (row < n && kk < k) {
+      const U4 v = *reinterpret_cast<const U4*>(wq + (int64_t)row * k + kk);
+      const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+      const int64_t gidx = (int64_t)row * ngroups + kk / group_size;
+      const float s = __half2float(scale[gidx]);
+      const float z = zp ? zp[gidx] : zp_const;
+      const bool exact = fabsf(s) >= 1e-5f;           // div_exact's domain; any other scale takes the IEEE division
+      const float rs = 1.f / s;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float w = bf16_bits_to_f32((uint16_t)((e & 1) ? (u[e / 2] >> 16) : (u[e / 2] & 0xffffu)));
+        const uint32_t code = (uint32_t)(exact ? (int32_t)rintf(div_exact(w, s, rs) + z) : int_code(w, s, z)) & 0xffu;
+        if (e < 4) lo |= code << (8 * e); else hi |= code << (8 * (e - 4));
+      }
+    }
+    tile[r][c] = U2{lo, hi};
+  }
+  __syncthreads();
+  const int words = n / 8;
+  for (int t = threadIdx.x; t < (AWQ_TN / 8) * (AWQ_TK / 8); t += 256) {
+    const int j = t % (AWQ_TN / 8), c = t / (AWQ_TN / 8);
+    const int oj = row0 / 8 + j, kk = k0 + c * 8;
+    if (oj >= words || kk >= k) continue;
+    uint32_t acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const U2 v = tile[j * 8 + i][c];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {                   // sum of shifted int32 lanes, wraps as the reference's does
+        const int32_t code = (int32_t)(int8_t)(((e < 4) ? (v.x >> (8 * e)) : (v.y >> (8 * (e - 4)))) & 0xffu);
+        acc[e] += ((uint32_t)code) << kAwqShift[i];
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) qweight[(int64_t)(kk + e) * words + oj] = (int32_t)acc[e];
+  }
+}
+
+// qzeros [G, N/8]: the zero-points of columns 8j .. 8j+7 in the same nibble order (a constant fills every nibble);
+// scales [G, N] = scale^T
+__global__ void awq_zeros_scales_kernel(const __half* __restrict__ scale, const float* __restrict__ zp, int zp_const, int n,
+                                        int ngroups, int32_t* __restrict__ qzeros, __half* __restrict__ scales_t) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)n * ngroups) return;
+  const int gi = (int)(idx / n), row = (int)(idx % n);
+  scales_t[idx] = scale[(int64_t)row * ngroups + gi];
+  if (row % 8 == 0) {
+    uint32_t acc = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (zp) acc += ((uint32_t)(int32_t)zp[(int64_t)(row + i) * ngroups + gi]) << kAwqShift[i];
+      else acc |= ((uint32_t)zp_const) << (4 * i);
+    }
+    qzeros[(int64_t)gi * (n / 8) + row / 8] = (int32_t)acc;
+  }
+}
+
+// inverse (dequantize_gemm, export_to_awq/utils.py:45-101): W'[N,K] = (code - zero) * scale
+__global__ void unpack_awq_kernel(const int32_t* __restrict__ qweight, const int32_t* __restrict__ qzeros,
+                                  const __half* __restrict__ scales_t, int n, int k, int group_size,
+                                  uint16_t* __restrict__ w_out, int32_t* __restrict__ codes) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)n * k) return;
+  const int row = (int)(idx % n), kk = (int)(idx / n), gi = kk / group_size;
+  const int sh = kAwqShift[row % 8];
+  const int32_t code = (int32_t)((((uint32_t)qweight[(int64_t)kk * (n / 8) + row / 8]) >> sh) & 15u);
+  const int32_t z = (int32_t)((((uint32_t)qzeros[(int64_t)gi * (n / 8) + row / 8]) >> sh) & 15u);
+  if (codes) codes[(int64_t)row * k + kk] = code;
+  if (w_out) w_out[(int64_t)row * k + kk] = f32_to_bf16_bits((float)(code - z) * __half2float(scales_t[(int64_t)gi * n + row]));
+}
+
 // ---- FP4: nibble = first-argmin over {0,.5,1,1.5,2,3,4,6} | signbit<<3 ; low nibble = even k
 template <bool IN_BF16_MATH>
 __device__ __forceinline__ uint32_t e2m1_nibble(float x) {
@@ -357,6 +447,40 @@ extern "C" int ar_unpack_int(const int32_t* qweight, const int32_t* qzeros, cons
   const int64_t total = (int64_t)n * k;
   unpack_int_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       qweight, qzeros, (const __half*)scales_t, n, k, bits, group_size, zp_minus_one, (uint16_t*)w_out, codes);
+  AR_CHECK_LAUNCH();
+  return AR_OK;
+}
+
+extern "C" int ar_pack_awq(const void* wq, const void* scale, const float* zp, int zp_const, int n, int k, int group_size,
+                           int32_t* qweight, int32_t* qzeros, void* scales_t, void* stream) {
+  AR_REQUIRE(wq && scale && qweight && qzeros && scales_t, AR_E_BADARG, "null pointer");
+  AR_REQUIRE(n > 0 && k > 0, AR_E_BADARG, "empty weight (n=%d k=%d)", n, k);
+  if (group_size == -1) group_size = k;
+  AR_REQUIRE(group_size > 0 && k % group_size == 0, AR_E_BADARG, "in_features (%d) shape mismatch", k);
+  AR_REQUIRE(n % 8 == 0, AR_E_BADARG, "out_features (%d) shape mismatch", n);
+  AR_REQUIRE(group_size % 8 == 0, AR_E_UNSUPPORTED, "awq pack needs group_size %% 8 == 0 (group_size=%d)", group_size);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((k + AWQ_TK - 1) / AWQ_TK, (n + AWQ_TN - 1) / AWQ_TN);
+  AR_REQUIRE(grid.y <= 65535u, AR_E_UNSUPPORTED, "awq pack: n=%d too large", n);
+  pack_awq_kernel<<<grid, 256, 0, st>>>((const uint16_t*)wq, (const __half*)scale, zp, (float)zp_const, n, k, group_size, qweight);
+  AR_CHECK_LAUNCH();
+  const int ngroups = k / group_size;
+  const int64_t total = (int64_t)n * ngroups;
+  awq_zeros_scales_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const __half*)scale, zp, zp_const, n, ngroups,
+                                                                          qzeros, (__half*)scales_t);
+  AR_CHECK_LAUNCH();
+  return AR_OK;
+}
+
+extern "C" int ar_unpack_awq(const int32_t* qweight, const int32_t* qzeros, const void* scales_t, int n, int k,
+                             int group_size, void* w_out, int32_t* codes, void* stream) {
+  AR_REQUIRE(qweight && qzeros && scales_t && (w_out || codes), AR_E_BADARG, "null pointer");
+  if (group_size == -1) group_size = k;
+  AR_REQUIRE(n > 0 && k > 0 && group_size > 0 && k % group_size == 0 && n % 8 == 0, AR_E_BADARG,
+             "awq unpack: n=%d k=%d group_size=%d", n, k, group_size);
+  const int64_t total = (int64_t)n * k;
+  unpack_awq_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      qweight, qzeros, (const __half*)scales_t, n, k, group_size, (uint16_t*)w_out, codes);
   AR_CHECK_LAUNCH();
   return AR_OK;
 }

@@ -18,7 +18,8 @@ LAUNCHES = [0]
 _KERNELS_PER_CALL = {"ar_group_minmax": 1, "ar_absmax": 1, "ar_nv_global_scale": 1, "ar_qdq_fwd": 1, "ar_qdq_bwd": 1,
                      "ar_gemm_bf16": 1, "ar_fq_linear_fwd": 2, "ar_fq_linear_bwd_dx": 1, "ar_fq_linear_bwd_dw": 1,
                      "ar_mse_fwd_bwd": 1, "ar_best_update": 1, "ar_sched_load": 1, "ar_iter_advance": 1, "ar_signsgd_step": 1, "ar_gather_rows": 1,
-                     "ar_pack_int": 3, "ar_unpack_int": 1, "ar_pack_fp4_nv": 1, "ar_pack_fp4_mx": 1, "ar_unpack_fp4": 1}
+                     "ar_pack_int": 3, "ar_unpack_int": 1, "ar_pack_awq": 2, "ar_unpack_awq": 1,
+                     "ar_pack_fp4_nv": 1, "ar_pack_fp4_mx": 1, "ar_unpack_fp4": 1}
 
 
 def _check(rc, what):
@@ -350,6 +351,36 @@ def unpack_int(qweight, qzeros, scales_t, n, k, bits, group_size, zp_minus_one, 
     codes = torch.empty(n, k, dtype=torch.int32, device=qweight.device) if want_codes else None
     _check(_lib.load().ar_unpack_int(_p(qweight), _p(qzeros), _p(scales_t), n, k, bits, g, int(zp_minus_one), _p(w),
                                          _p(codes), _stream()), "ar_unpack_int")
+    return w, codes
+
+
+def pack_awq(wq, scale_f16, zp, group_size, zp_const=0):
+    """AWQ GEMM layout, 4 bit -> qweight i32 [K,N/8], qzeros i32 [G,N/8], scales fp16 [G,N].  `zp` fp32 [N,G], or None
+    for a symmetric layer (`zp_const` fills every nibble).  Shapes the layout cannot hold raise the reference's
+    ValueError (export_to_awq/utils.py:153-158)."""
+    _want(wq, torch.bfloat16, "wq")
+    _want(scale_f16, torch.float16, "scale")
+    _want(zp, torch.float32, "zp")
+    n, k = wq.shape
+    g = k if group_size == -1 else group_size
+    if g <= 0 or k % g != 0:
+        raise ValueError(f"in_features ({k}) shape mismatch")
+    if n % 8 != 0:
+        raise ValueError(f"out_features ({n}) shape mismatch")
+    dev = wq.device
+    qweight = torch.empty(k, n // 8, dtype=torch.int32, device=dev)
+    qzeros = torch.empty(k // g, n // 8, dtype=torch.int32, device=dev)
+    scales_t = torch.empty(k // g, n, dtype=torch.float16, device=dev)
+    _check(_lib.load().ar_pack_awq(_p(wq), _p(scale_f16), _p(zp), int(zp_const), n, k, g, _p(qweight), _p(qzeros),
+                                   _p(scales_t), _stream()), "ar_pack_awq")
+    return qweight, qzeros, scales_t
+
+
+def unpack_awq(qweight, qzeros, scales_t, n, k, group_size, want_codes=False):
+    w = torch.empty(n, k, dtype=torch.bfloat16, device=qweight.device)
+    codes = torch.empty(n, k, dtype=torch.int32, device=qweight.device) if want_codes else None
+    _check(_lib.load().ar_unpack_awq(_p(qweight), _p(qzeros), _p(scales_t), n, k, group_size, _p(w), _p(codes), _stream()),
+           "ar_unpack_awq")
     return w, codes
 
 

@@ -140,7 +140,8 @@ def restore_block(block: nn.Module, snap: dict, scheme_for) -> list:
         if rec["kind"] == "packed":
             bias = rec["buffers"].get("bias")
             bufs = {k: v for k, v in rec["buffers"].items() if k != "bias"}
-            set_module(block, name, QuantLinear(rec["in_features"], rec["out_features"], scheme_for(name, lin), bufs, bias))
+            set_module(block, name, QuantLinear(rec["in_features"], rec["out_features"], scheme_for(name, lin), bufs, bias,
+                                                persist_g_idx="g_idx" not in rec.get("non_persistent", ["g_idx"])))
         else:
             lin.weight.data = rec["weight"].to(lin.weight.dtype)
             for a in _LAYER_ATTRS:

@@ -291,6 +291,22 @@ int ar_unpack_int(const int32_t* qweight, const int32_t* qzeros, const void* sca
                   int group_size, int zp_minus_one, void* w_bf16, int32_t* codes_or_null, void* stream);
 
 /*
+ * AWQ "GEMM" layout, 4 bit -- WQLinear_GEMM.from_linear, auto_round/export/export_to_awq/utils.py:197-273.  Words run
+ * along N (ar_pack_int packs along K): word j of row k holds the codes of output columns 8j .. 8j+7, column 8j+i at bit
+ * 4 * [0,4,1,5,2,6,3,7][i]; qzeros packs the zero-points the same way (zp NULL: zp_const fills every nibble).
+ * in:  wq bf16 [N,K], scale fp16 [N,G] (G = K / group_size; group_size -1 = K), zp fp32 [N,G] or NULL (+zp_const)
+ * out: qweight i32 [K, N/8]; qzeros i32 [G, N/8]; scales fp16 [G, N]
+ * AR_E_BADARG when K % group_size != 0 or N % 8 != 0 (the reference's "shape mismatch"); AR_E_UNSUPPORTED when
+ * group_size % 8 != 0.
+ */
+int ar_pack_awq(const void* wq_bf16, const void* scale_f16, const float* zp, int zp_const, int n, int k, int group_size,
+                int32_t* qweight, int32_t* qzeros, void* scales_f16, void* stream);
+/* inverse (tests / round trips): W'[N,K] bf16 = (code - zero) * scale, as dequantize_gemm (utils.py:45-101); either
+ * output may be NULL */
+int ar_unpack_awq(const int32_t* qweight, const int32_t* qzeros, const void* scales_f16, int n, int k, int group_size,
+                  void* w_bf16_or_null, int32_t* codes_or_null, void* stream);
+
+/*
  * FP4 pack -- auto_round/export/export_to_autoround/qlinear_fp.py:141-193, :235-265
  * nv: weight_packed u8 [N,K/2], weight_scale e4m3 bytes [N,K/16]; scale_f32 = layer.scale, gscale device scalar
  * mx: weight_packed u8 [N,K/2], weight_scale u8 [N,K/32] = clamp(e+127,0,255); exp_bf16 = layer.scale
