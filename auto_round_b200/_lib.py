@@ -29,24 +29,17 @@ SIGNATURES = {
     "ar_nv_global_scale": [_P, _P, _P],
     "ar_qdq_fwd": [_QS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "ar_qdq_bwd": [_QS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P],
-    "ar_qdq_int_sym_fwd": [_QS, _P, _P, _P, _P, _P, _P, _P, _P, _P],
-    "ar_qdq_int_asym_fwd": [_QS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
-    "ar_qdq_mx_fp4_fwd": [_QS, _P, _P, _P, _P, _P, _P],
-    "ar_qdq_nv_fp4_fwd": [_QS, _P, _P, _P, _P, _P, _P, _P],
     "ar_gemm_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _L, _P, _P],
     "ar_gemm_bf16_grouped": [_P, _P, _P, _I, _I, _I, _I, _I, _I, _L, _L, _L, _I, _I, _P, _P, _I, _I, _P],
     "ar_moe_route": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "ar_moe_gather": [_P, _P, _P, _I, _I, _I, _P, _P],
     "ar_moe_combine": [_P, _P, _P, _P, _I, _I, _I, _P, _P],
     "ar_moe_rowdot": [_P, _P, _P, _I, _I, _I, _P, _P],
-    "ar_fq_linear_fwd": [_QS, _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "ar_fq_linear_bwd_dx": [_QS, _P, _L, _P, _P, _P],
-    "ar_fq_linear_bwd_dw": [_QS, _P, _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _P],
     "ar_fq_update": [_QS, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P],
     "ar_wq_decode": [_QS, _P, _L, _I, _P, _P],
     "ar_mse_fwd_bwd": [_P, _P, _P, _L, _L, _F, _F, _P, _P, _P],
     "ar_best_update": [_P, _D, _D, _I, _P, _P, _P, _P, _P, _P],
-    "ar_signsgd_step": [_P, _P, _I, _P, _P, _P, _P, _I, _P, _L, _L, _F, _P],
     "ar_sched_load": [_P, _P, _P, _I, _P, _P, _P, _P],
     "ar_iter_advance": [_P, _P],
     "ar_rmsnorm_fwd": [_P, _P, _F, _L, _I, _P, _P, _P],

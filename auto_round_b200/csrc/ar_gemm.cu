@@ -3,23 +3,20 @@
 //   D[M,N] = A[M,K] · B[N,K]ᵀ ,  fp32 accumulate in registers, operands staged by TMA into 128B-swizzled smem.
 //
 // One persistent CTA per SM (132 on an H100 SXM), warp-specialised:
-//   warps 0..7  two consumer warpgroups: warpgroup w issues wgmma.m64n{BN}k16 for rows [64w, 64w+64) of the 128 x BN
+//   warps 0..7  two consumer warpgroups: warpgroup w issues wgmma.m64n256k16 for rows [64w, 64w+64) of the 128 x 256
 //               tile, then runs the epilogue of its own rows
 //   warp 8      TMA producer   (one elected lane; mbarrier full/empty ring; keeps loading the next tile's stages while
 //                               the consumers run the epilogue of the current one)
-// Tile width BN per epilogue: EPI_STORE uses 128 x 256 tiles (m64n256k16 reads 17 % fewer smem bytes per FLOP than
-// m64n128k16, and each staged A slab feeds twice the output columns); EPI_DW keeps 128 x 128 tiles because its fp32
-// staging tile would not fit beside a 128 x 256 operand ring.
+// Tiles are 128 x 256: m64n256k16 reads 17 % fewer smem bytes per FLOP than m64n128k16, and each staged A slab feeds
+// twice the output columns.
 // Each operand may be K-major (reduction dim contiguous) or MN-major (row dim contiguous), which covers the
 // three GEMMs of a linear without any transposed copies (wgmma's transpose bits read MN-major bf16 directly):
 //   forward   Y  = X  · Wqᵀ      A = X  [T,K]  K-major      B = Wq [N,K]  K-major
 //   grad-in   dX = dY · Wq       A = dY [T,N]  K-major      B = Wq [N,K]  as [K_out, N_red]: MN-major
 //   grad-w    dW = dYᵀ· X        A = dY [T,N]  as [N_out, T_red]: MN-major   B = X [T,K] as [K_out, T_red]: MN-major
-// Epilogues:
-//   EPI_STORE  fp32 registers -> (+bias) -> bf16 -> global, straight from each warpgroup's accumulators (a quad
-//              transpose gives 16-byte stores; clipped to the problem); no smem staging and no consumer barrier
-//   EPI_DW     fp32 dWq tile -> smem staging tile -> fake-quant backward in registers -> dV (fp32), d min/max_scale per group; the
-//              dWq matrix itself is never written (auto_round: autograd through wrapper.py:273-290)
+// Epilogue: fp32 registers -> (+bias) -> bf16 -> global, straight from each warpgroup's accumulators (a quad transpose
+// gives 16-byte stores; clipped to the problem); no smem staging and no consumer barrier.  The fake-quant backward of
+// the grad-w GEMM's bf16 dWq runs in the per-layer update kernel (ar_fq_update, ar_qdq.cu).
 // FLOPs per launch = 2*M*N*K; roofline = dense bf16 tensor peak (MEASURED_PEAKS.json: bf16_tflops).
 #include <cuda.h>
 
@@ -28,13 +25,12 @@
 #include <atomic>
 #include <mutex>
 
-#include "ar_qdq_math.cuh"
+#include "ar_common.cuh"
 
 namespace ar {
 
 constexpr int BLOCK_M = 128;
-constexpr int kStoreBN = 256;         // tile width of the EPI_STORE launches
-constexpr int kDwBN = 128;            // tile width of the EPI_DW launches
+constexpr int BLOCK_N = 256;
 constexpr int BLOCK_K = 64;           // 64 bf16 = 128 B = one swizzle atom row
 constexpr int WGMMA_K = 16;
 constexpr int kStages = 4;
@@ -42,8 +38,6 @@ constexpr int kConsumerThreads = 256; // two warpgroups
 constexpr int kProducerWarp = 8;
 constexpr int kNumThreads = kConsumerThreads + 32;
 constexpr int kTableRows = 256;       // row granularity of the MoE routing tables (GROUP_M entries, padded segments)
-
-enum { EPI_STORE = 0, EPI_DW = 1 };
 
 // ------------------------------------------------------------------------------------------------ PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -94,7 +88,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -116,32 +109,8 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
   return d;
 }
 
-// D(64 x 128, fp32, registers) += A(64 x 16) · B(128 x 16)ᵀ.  Fragment of thread (warp w of the warpgroup, lane l):
-// d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
-  asm volatile(
-      "{\n"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, 1, 1, 1, %66, %67;\n"
-      "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
-        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
-        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
-        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
-        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
-      : "memory");
-}
-
-// D(64 x 256, fp32, registers) += A(64 x 16) · B(256 x 16)ᵀ; same fragment layout as m64n128k16 with j in [0, 32).
+// D(64 x 256, fp32, registers) += A(64 x 16) · B(256 x 16)ᵀ.  Fragment of thread (warp w of the warpgroup, lane l):
+// d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e], j in [0, 32).
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
@@ -178,31 +147,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
       : "memory");
 }
 
-template <int BN, int TA, int TB>
-__device__ __forceinline__ void wgmma_tile_k16(float (&d)[BN / 2], uint64_t desc_a, uint64_t desc_b) {
-  if constexpr (BN == 256) wgmma_m64n256k16<TA, TB>(d, desc_a, desc_b);
-  else wgmma_m64n128k16<TA, TB>(d, desc_a, desc_b);
-}
-
 // ---------------------------------------------------------------------------------------- kernel params
-struct DwParams {                 // EPI_DW: fake-quant backward inputs/outputs
-  const uint16_t* w;              // bf16 [N,K]
-  const float* v;                 // fp32 [N,K] or null
-  const float* mn;                // [G] or null
-  const float* mx;                // [G] or null
-  const uint16_t* wmin;           // bf16 [G] (int types)
-  const uint16_t* wmax;
-  const float* gscale;            // nv
-  void* dv;                       // [N,K] fp32, or bf16 when dv_bf16 (halves the all-reduce volume under DP)
-  float* dmin;                    // [G] or null
-  float* dmax;                    // [G] or null
-  int bits;
-  float thr;
-  int accumulate;
-  int dv_bf16;
-  const float* init;              // ar_qspec::init_scale (alg_ext) or null
-};
-
 // Grouped (ragged per-expert) GEMMs of the MoE path: tiles are resolved through small device-side tables written by the
 // routing kernel of the same iteration (ar_moe_route), so launches stay static and graph-capturable.
 //   GROUP_M  forward / grad-in of all experts in one launch: A rows are the routed tokens sorted by expert, every expert's
@@ -233,31 +178,28 @@ struct GemmParams {
   // host-only (grouped launches): extents of the tensor maps when they differ from the logical problem, and the tile bound
   int a_rows_map, b_rows_map, b_k_map, d_rows_map, max_tiles;
   int m_tiles, n_tiles;
-  uint16_t* d;                    // EPI_STORE: bf16 output, row pitch ldd, d_rows x n
+  uint16_t* d;                    // bf16 output, row pitch ldd, d_rows x n
   int64_t ldd;
   int d_rows;
-  const uint16_t* bias;           // EPI_STORE, optional [n]
+  const uint16_t* bias;           // optional [n]
   unsigned int* tile_ctr;         // dynamic tile scheduler: ticket counter of this launch (0 at launch, reset to 0 at exit)
-  DwParams dw;
+  // Unused: keeps the parameter block above 128 bytes.  At 128 bytes or less nvcc reads it through uniform registers and
+  // schedules every instantiation differently (155-159 registers instead of 156-158); the rates in DESIGN §4.1 were
+  // measured on the code generated for the larger block.
+  uint8_t pad[16];
 };
+static_assert(sizeof(GemmParams) > 128, "see GemmParams::pad");
 
-// Staging tile of the EPI_DW epilogue: fp32 [BLOCK_M][kStageLd]; the pad of 8 floats makes the float2 fragment stores
-// of a half-warp (4 rows x 4 column pairs) hit 32 distinct banks.  EPI_STORE has no staging tile.
-constexpr int kStageLd = kDwBN + 8;
-template <int BN, bool STAGED>
-struct SmemLayout {
+// Shared memory: the 4 x 48 KB operand ring (192 KB), then the mbarriers and the ticket slots.
+struct Smem {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;       // 16 KB
-  static constexpr int kBBytes = BN * BLOCK_K * 2;            // 16 KB (BN 128) or 32 KB (BN 256)
+  static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;       // 32 KB
   static constexpr int kAOff = 0;
   static constexpr int kBOff = kStages * kABytes;
-  static constexpr int kCOff = kBOff + kStages * kBBytes;
-  static constexpr int kCBytes = STAGED ? BLOCK_M * kStageLd * 4 : 0;   // 68 KB
-  static constexpr int kBarOff = kCOff + kCBytes;
+  static constexpr int kBarOff = kBOff + kStages * kBBytes;
   static constexpr int kTotal = kBarOff + 512 + 1024;         // + slack to align the base to 1024 B (SWIZZLE_128B atoms)
   static_assert(kTotal <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
 };
-using StoreSmem = SmemLayout<kStoreBN, false>;                // 4 x 48 KB ring = 192 KB
-using DwSmem = SmemLayout<kDwBN, true>;                       // 4 x 32 KB ring + 68 KB staging = 196 KB
 constexpr int kSchedSlots = 8;
 
 // tile order: groups of 8 M-tiles sweep all N-tiles, so the concurrent CTAs share A/B tiles in L2
@@ -272,7 +214,7 @@ __device__ __forceinline__ void tile_coords(int t, int m_tiles, int n_tiles, int
   nt = in / gm;
 }
 
-template <int BN, bool B_MN>
+template <bool B_MN>
 __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int m_tiles, int num_kb_static) {
   TileInfo ti;
   int mt, nt;
@@ -282,7 +224,7 @@ __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int
     tile_coords(t - ae * per, p.m_tiles, p.n_tiles, mt, nt);
     const int e = p.grp.table[3 * ae], koff = p.grp.table[3 * ae + 1], klen = p.grp.table[3 * ae + 2];
     ti.m0 = mt * BLOCK_M;
-    ti.n0 = nt * BN;
+    ti.n0 = nt * BLOCK_N;
     ti.d_m0 = e * p.grp.d_group_rows + ti.m0;
     ti.d_n0 = ti.n0;
     ti.a_koff = koff;
@@ -291,7 +233,7 @@ __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int
     return ti;
   }
   tile_coords(t, m_tiles, p.n_tiles, mt, nt);
-  ti.n0 = nt * BN;
+  ti.n0 = nt * BLOCK_N;
   ti.d_n0 = ti.n0;
   ti.a_koff = 0;
   ti.b_koff = 0;
@@ -309,143 +251,15 @@ __device__ __forceinline__ TileInfo resolve_tile(const GemmParams& p, int t, int
   return ti;
 }
 
-// ------------------------------------------------------------------------------------- dW fused epilogue
-// Thread owns output row `row` (= output feature n) and walks SPAN staged columns (= input features k, whole groups) in
-// chunks of 32.  `acc` points at the staged fp32 accumulator of that row, column col0 - (tile's first column).
-template <class Ctx, int G, bool IS_FP4, int SPAN>
-__device__ __forceinline__ void epilogue_dw(const GemmParams& p, const float* acc_row, int row, int col0) {
-  const DwParams& d = p.dw;
-  const int N = p.m, K = p.n;                     // GEMM "m" is the layer's N (out features), GEMM "n" its K
-  if (row >= N) return;
-  const int gpr = K / G;
-  Ctx ctx;
-  ctx.init(d.bits);
-  GroupIn gi;
-  gi.thr = d.thr;
-  gi.gscale = (IS_FP4 && d.gscale) ? *d.gscale : 0.f;
-  GroupAcc acc;
-  // W / V of chunk c+1 are requested before chunk c is processed (software prefetch: with short reductions, e.g. the
-  // per-GPU share of a data-parallel batch, the epilogue and not the MMA main loop bounds the grad-w GEMM)
-  U4 wr[4];
-  float4 vr[8];
-  auto fetch = [&](int c) {
-    const int k0 = col0 + c * 32;
-    if (k0 < K) {
-      const int64_t off = (int64_t)row * K + k0;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) wr[j] = reinterpret_cast<const U4*>(d.w + off)[j];
-      if (d.v) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) vr[j] = reinterpret_cast<const float4*>(d.v + off)[j];
-      }
-    }
-  };
-  fetch(0);
-#pragma unroll 1
-  for (int c = 0; c < SPAN / 32; ++c) {
-    const int k0 = col0 + c * 32;
-    if (k0 >= K) break;
-    float w[32], v[32];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint32_t u[4] = {wr[j].x, wr[j].y, wr[j].z, wr[j].w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        w[j * 8 + 2 * i] = bf16_bits_to_f32((uint16_t)(u[i] & 0xffffu));
-        w[j * 8 + 2 * i + 1] = bf16_bits_to_f32((uint16_t)(u[i] >> 16));
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[4 * j] = d.v ? vr[j].x : 0.f; v[4 * j + 1] = d.v ? vr[j].y : 0.f;
-      v[4 * j + 2] = d.v ? vr[j].z : 0.f; v[4 * j + 3] = d.v ? vr[j].w : 0.f;
-    }
-    if (c + 1 < SPAN / 32) fetch(c + 1);
-    float r[32];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 q = reinterpret_cast<const float4*>(acc_row + c * 32)[j];
-      r[4 * j] = q.x; r[4 * j + 1] = q.y; r[4 * j + 2] = q.z; r[4 * j + 3] = q.w;
-    }
-    const int64_t off = (int64_t)row * K + k0;
-    float out[32];
-    constexpr int SUB = (G < 32) ? G : 32;         // elements of one group inside this chunk
-#pragma unroll
-    for (int s = 0; s < 32 / SUB; ++s) {
-      const int kk = k0 + s * SUB;
-      const int64_t gidx = (int64_t)row * gpr + kk / G;
-      if ((kk % G) == 0) {                         // group starts here: build its context
-        gi.mn = d.mn ? d.mn[gidx] : 1.f;
-        gi.mx = d.mx ? d.mx[gidx] : 1.f;
-        gi.has_init = (d.init != nullptr);
-        gi.init = d.init ? d.init[gidx] : 1.f;
-        if (IS_FP4) {
-          float am = 0.f;
-#pragma unroll
-          for (int i = 0; i < SUB; ++i) am = fmaxf(am, fabsf(w[s * SUB + i]));
-          gi.wmax = am; gi.wmin = 0.f;             // G <= 32 for fp4: the whole group is in registers
-        } else {
-          gi.wmin = bf16_bits_to_f32(d.wmin[gidx]);
-          gi.wmax = bf16_bits_to_f32(d.wmax[gidx]);
-        }
-        ctx.setup(gi);
-        acc = GroupAcc();
-      }
-#pragma unroll
-      for (int i = 0; i < SUB; ++i) ctx.bwd(w[s * SUB + i], v[s * SUB + i], r[s * SUB + i], out[s * SUB + i], acc);
-      if (((kk + SUB) % G) == 0) {                 // group complete
-        float gmn, gmx;
-        ctx.finish(acc, gi, gmn, gmx);
-        if (d.dmax) d.dmax[gidx] = d.accumulate ? d.dmax[gidx] + gmx : gmx;
-        if (d.dmin) d.dmin[gidx] = d.accumulate ? d.dmin[gidx] + gmn : gmn;
-      }
-    }
-    if (d.dv_bf16) {
-      uint16_t* o = reinterpret_cast<uint16_t*>(d.dv) + off;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float e[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) e[i] = out[8 * j + i];
-        if (d.accumulate) {
-          const U4 old = reinterpret_cast<const U4*>(o)[j];
-          const uint32_t u[4] = {old.x, old.y, old.z, old.w};
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            e[2 * i] += bf16_bits_to_f32((uint16_t)(u[i] & 0xffffu));
-            e[2 * i + 1] += bf16_bits_to_f32((uint16_t)(u[i] >> 16));
-          }
-        }
-        uint32_t pk[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) pk[i] = (uint32_t)f32_to_bf16_bits(e[2 * i]) | ((uint32_t)f32_to_bf16_bits(e[2 * i + 1]) << 16);
-        reinterpret_cast<U4*>(o)[j] = U4{pk[0], pk[1], pk[2], pk[3]};
-      }
-    } else {
-      float* o = reinterpret_cast<float*>(d.dv) + off;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 q = make_float4(out[4 * j], out[4 * j + 1], out[4 * j + 2], out[4 * j + 3]);
-        if (d.accumulate) {
-          const float4 old = reinterpret_cast<const float4*>(o)[j];
-          q.x += old.x; q.y += old.y; q.z += old.z; q.w += old.w;
-        }
-        reinterpret_cast<float4*>(o)[j] = q;
-      }
-    }
-  }
-}
-
 // bf16 store epilogue straight from one warpgroup's accumulators.  Thread (warp w of the warpgroup, lane l) holds
 // D[16w + l/4 + 8h][8j + 2(l%4) + e] in acc[4j + 2h + e]; `row0` is the output row of h = 0.  After the bias and the
 // rounding to bf16 pairs, a 4 x 4 transpose inside each quad (two shfl.xor rounds) hands lane q of the quad the 8
 // consecutive columns 8(4b + q) .. +7 of its row, so each 16-byte store of a warp writes 8 rows x 64 contiguous bytes.
-template <int BN>
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float (&acc)[BN / 2], int row0, int n0, int lane) {
+__device__ __forceinline__ void epilogue_store(const GemmParams& p, const float (&acc)[BLOCK_N / 2], int row0, int n0, int lane) {
   const int q = lane & 3;
   const bool odd = (q & 1) != 0, hi = (q & 2) != 0;
 #pragma unroll
-  for (int b = 0; b < BN / 32; ++b) {
+  for (int b = 0; b < BLOCK_N / 32; ++b) {
     uint32_t v[2][4];                                      // [h][s]: bf16 pair of columns 8(4b + s) + 2q, +1
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
@@ -495,11 +309,10 @@ __device__ __forceinline__ void epilogue_store(const GemmParams& p, const float 
 // when NCCL kernels of the data-parallel exchange hold a few SMs while a GEMM launches (they cannot co-reside with a 200 KB
 // CTA).  With tickets, late CTAs simply find the queue empty.  Ticket order = rasterised tile order, so concurrently
 // running CTAs still work on neighbouring tiles (L2 reuse).  The CTA that draws the last terminal ticket resets the counter.
-template <int BN, bool A_MN, bool B_MN, int EPI, class Ctx, int G, bool IS_FP4>
+template <bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
-  static_assert(EPI == EPI_STORE || BN == kDwBN, "the EPI_DW staging tile is 128 columns wide");
-  using L = SmemLayout<BN, EPI == EPI_DW>;
+  using L = Smem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -539,7 +352,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         mbar_arrive(&sfull[slot]);
         if (t >= num_tiles) break;
         t_next = (int)atomicAdd(p.tile_ctr, 1u);           // next ticket: in flight while this tile's loads are issued
-        const TileInfo ti = resolve_tile<BN, B_MN>(p, t, m_tiles_dyn, num_kb);
+        const TileInfo ti = resolve_tile<B_MN>(p, t, m_tiles_dyn, num_kb);
         for (int kb = 0; kb < ti.num_kb; ++kb, ++it) {
           const uint32_t s = it % kStages, sph = (it / kStages) & 1u;
           mbar_wait(&empty[s], sph ^ 1u);
@@ -555,10 +368,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
               tma_load_2d(sa + i * (64 * BLOCK_K * 2), &map_a, &full[s], ti.m0 + i * 64, ti.a_koff + k0);
           }
           if (!B_MN) {
-            tma_load_2d(sb, &map_b, &full[s], ti.b_koff + k0, ti.n0);                 // box {64 k, BN n}
+            tma_load_2d(sb, &map_b, &full[s], ti.b_koff + k0, ti.n0);                 // box {64 k, 256 n}
           } else {
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i)
+            for (int i = 0; i < BLOCK_N / 64; ++i)
               tma_load_2d(sb + i * (64 * BLOCK_K * 2), &map_b, &full[s], ti.n0 + i * 64, ti.b_koff + k0);
           }
         }
@@ -583,11 +396,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       __syncwarp();
       if (lane == 0) mbar_arrive(&sempty[slot]);
       if (t >= num_tiles) break;
-      const TileInfo ti = resolve_tile<BN, B_MN>(p, t, m_tiles_dyn, num_kb);
+      const TileInfo ti = resolve_tile<B_MN>(p, t, m_tiles_dyn, num_kb);
 
-      float acc[BN / 2];
+      float acc[BLOCK_N / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
       uint32_t prev = 0;
       for (int kb = 0; kb < ti.num_kb; ++kb, ++it) {
         const uint32_t s = it % kStages, sph = (it / kStages) & 1u;
@@ -597,8 +410,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
-          wgmma_tile_k16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, make_smem_desc(sa + k * a_kstep, a_lbo, 1024),
-                                                         make_smem_desc(sb + k * b_kstep, b_lbo, 1024));
+          wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, make_smem_desc(sa + k * a_kstep, a_lbo, 1024),
+                                                      make_smem_desc(sb + k * b_kstep, b_lbo, 1024));
         wgmma_commit();
         wgmma_wait<1>();                                   // the previous stage's MMAs have retired: hand it back
         if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
@@ -607,27 +420,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       wgmma_wait<0>();
       if (ti.num_kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
 
-      if constexpr (EPI == EPI_DW) {
-        float* stage = reinterpret_cast<float*>(smem + L::kCOff);
-        consumer_bar_sync();                               // the previous tile's epilogue is done reading the staging tile
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int col = 8 * j + 2 * (lane & 3);
-          const int r0 = wg * 64 + wrow;
-          *reinterpret_cast<float2*>(stage + r0 * kStageLd + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(stage + (r0 + 8) * kStageLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        consumer_bar_sync();
-        constexpr int SPAN = (G > 64) ? G : 64;            // whole groups per thread
-        constexpr int kUnits = BLOCK_M * (BN / SPAN);
-        if (ctid < kUnits) {
-          const int r = ctid % BLOCK_M, c = (ctid / BLOCK_M) * SPAN;
-          epilogue_dw<Ctx, G, IS_FP4, SPAN>(p, stage + r * kStageLd + c, ti.d_m0 + r, ti.d_n0 + c);
-        }
-      } else {
-        // each warpgroup stores its own 64 rows and moves on to the next ticket: no consumer-wide barrier
-        epilogue_store<BN>(p, acc, ti.d_m0 + wg * 64 + wrow, ti.d_n0, lane);
-      }
+      // each warpgroup stores its own 64 rows and moves on to the next ticket: no consumer-wide barrier
+      epilogue_store(p, acc, ti.d_m0 + wg * 64 + wrow, ti.d_n0, lane);
     }
   }
 }
@@ -650,9 +444,20 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
+// cuTensorMapEncodeTiled is a driver call and fails with CUDA_ERROR_INVALID_CONTEXT in a thread that has no current
+// context.  A thread that has made no runtime call yet has none, and PyTorch's autograd device threads start that way
+// (they skip cudaSetDevice when the device already matches), so the first GEMM of a backward can come from such a thread.
+// cudaSetDevice makes the device's primary context current; once per thread.
+static void ensure_context() {
+  thread_local bool done = false;
+  int dev = 0;
+  if (!done && cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) done = true;
+}
+
 // 2-D bf16 tensor map: dim0 = contiguous dimension.  box = {box0, box1}, 128B swizzle (box0 * 2 B == 128 B).
 static int make_map(CUtensorMap* map, const void* ptr, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
                     uint32_t box1) {
+  ensure_context();
   PFN_encodeTiled enc = get_encode();
   AR_REQUIRE(enc != nullptr, AR_E_DRIVER, "cuTensorMapEncodeTiled entry point not available");
   AR_REQUIRE(((uintptr_t)ptr & 15u) == 0, AR_E_BADARG, "TMA operand must be 16-byte aligned");
@@ -701,12 +506,11 @@ static unsigned int* next_tile_counter() {
   return base[dev] + (next.fetch_add(1) % kCtrSlots);
 }
 
-template <bool A_MN, bool B_MN, int EPI, class Ctx, int G, bool IS_FP4>
+template <bool A_MN, bool B_MN>
 static int launch(const void* a, const void* b, void* d, int m, int n, int k, int64_t lda, int64_t ldb, int64_t ldd,
                   const GemmParams& base, cudaStream_t st) {
-  constexpr int BN = (EPI == EPI_STORE) ? kStoreBN : kDwBN;
-  using L = SmemLayout<BN, EPI == EPI_DW>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, Ctx, G, IS_FP4>;
+  using L = Smem;
+  auto kern = gemm_kernel<A_MN, B_MN>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
@@ -721,31 +525,27 @@ static int launch(const void* a, const void* b, void* d, int m, int n, int k, in
   if (rc) return rc;
   const uint64_t b_rows = base.b_rows_map > 0 ? (uint64_t)base.b_rows_map : (uint64_t)n;
   const uint64_t b_k = base.b_k_map > 0 ? (uint64_t)base.b_k_map : (uint64_t)k;
-  if (!B_MN) rc = make_map(&mb, b, b_k, b_rows, (uint64_t)ldb, 64, BN);
+  if (!B_MN) rc = make_map(&mb, b, b_k, b_rows, (uint64_t)ldb, 64, BLOCK_N);
   else rc = make_map(&mb, b, b_rows, b_k, (uint64_t)ldb, 64, BLOCK_K);
   if (rc) return rc;
+  AR_REQUIRE(((uintptr_t)d & 15u) == 0, AR_E_BADARG, "GEMM output must be 16-byte aligned");
+  AR_REQUIRE(ldd % 8 == 0, AR_E_BADARG, "GEMM output leading dimension must be a multiple of 8 elements (got %lld)",
+             (long long)ldd);
   GemmParams p = base;
-  if (EPI == EPI_STORE) {
-    AR_REQUIRE(((uintptr_t)d & 15u) == 0, AR_E_BADARG, "GEMM output must be 16-byte aligned");
-    AR_REQUIRE(ldd % 8 == 0, AR_E_BADARG, "GEMM output leading dimension must be a multiple of 8 elements (got %lld)",
-               (long long)ldd);
-    p.d = (uint16_t*)d;
-    p.ldd = ldd;
-    p.d_rows = base.d_rows_map > 0 ? base.d_rows_map : m;
-  }
+  p.d = (uint16_t*)d;
+  p.ldd = ldd;
+  p.d_rows = base.d_rows_map > 0 ? base.d_rows_map : m;
   p.m = m; p.n = n; p.k = k;
   p.tile_ctr = next_tile_counter();
   AR_REQUIRE(p.tile_ctr != nullptr, AR_E_DRIVER, "tile counter symbol not available on this device");
   p.m_tiles = (m + BLOCK_M - 1) / BLOCK_M;
-  p.n_tiles = (n + BN - 1) / BN;
+  p.n_tiles = (n + BLOCK_N - 1) / BLOCK_N;
   const int tiles = base.max_tiles > 0 ? base.max_tiles : p.m_tiles * p.n_tiles;
   const int ctas = tiles < sm_count() ? tiles : sm_count();
   kern<<<(unsigned)ctas, kNumThreads, L::kTotal, st>>>(ma, mb, p);
   AR_CHECK_LAUNCH();
   return AR_OK;
 }
-
-struct NoCtx {};
 
 }  // namespace ar
 
@@ -758,10 +558,10 @@ extern "C" int ar_gemm_bf16(const void* a, const void* b, void* d, int m, int n,
   GemmParams p{};
   p.bias = (const uint16_t*)bias;
   cudaStream_t st = (cudaStream_t)stream;
-  if (!a_mn && !b_mn) return launch<false, false, EPI_STORE, NoCtx, 32, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
-  if (!a_mn && b_mn) return launch<false, true, EPI_STORE, NoCtx, 32, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
-  if (a_mn && !b_mn) return launch<true, false, EPI_STORE, NoCtx, 32, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
-  return launch<true, true, EPI_STORE, NoCtx, 32, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
+  if (!a_mn && !b_mn) return launch<false, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
+  if (!a_mn && b_mn) return launch<false, true>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
+  if (a_mn && !b_mn) return launch<true, false>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
+  return launch<true, true>(a, b, d, m, n, k, lda, ldb, ldd, p, st);
 }
 
 extern "C" int ar_gemm_bf16_grouped(const void* a, const void* b, void* d, int mode, int rows, int n, int k, int a_mn, int b_mn,
@@ -776,7 +576,7 @@ extern "C" int ar_gemm_bf16_grouped(const void* a, const void* b, void* d, int m
   p.grp.table = table;
   p.grp.num = num;
   cudaStream_t st = (cudaStream_t)stream;
-  const int n_tiles = (n + kStoreBN - 1) / kStoreBN;     // both grouped modes launch EPI_STORE instantiations
+  const int n_tiles = (n + BLOCK_N - 1) / BLOCK_N;
   if (mode == GROUP_M) {
     // D[rows, n] = A[rows, k] * B_e^T, e = expert of the row tile.  B stacked over experts: K-major [G * group_rows, k]
     // (forward: group_rows = n) or stored [G * group_rows, n] read MN-major with the reduction inside the expert's rows
@@ -787,10 +587,10 @@ extern "C" int ar_gemm_bf16_grouped(const void* a, const void* b, void* d, int m
     p.max_tiles = max_entries * (kTableRows / BLOCK_M) * n_tiles;
     if (!b_mn) {
       p.b_rows_map = group_rows * num_groups;
-      return launch<false, false, EPI_STORE, NoCtx, 32, false>(a, b, d, rows, n, k, lda, ldb, ldd, p, st);
+      return launch<false, false>(a, b, d, rows, n, k, lda, ldb, ldd, p, st);
     }
     p.b_k_map = group_rows * num_groups;
-    return launch<false, true, EPI_STORE, NoCtx, 32, false>(a, b, d, rows, n, k, lda, ldb, ldd, p, st);
+    return launch<false, true>(a, b, d, rows, n, k, lda, ldb, ldd, p, st);
   }
   // GROUP_K: D_e[n_out = `n`... ] -- here the logical problem per active expert is D[m = group_rows, n] = A^T B over that
   // expert's rows; A stored [rows, m] and B stored [rows, n] (both MN-major), D stacked [G * group_rows, n]
@@ -802,53 +602,11 @@ extern "C" int ar_gemm_bf16_grouped(const void* a, const void* b, void* d, int m
   p.grp.d_group_rows = group_rows;
   p.d_rows_map = group_rows * num_groups;
   p.max_tiles = max_entries * (group_rows / BLOCK_M) * n_tiles;
-  return launch<true, true, EPI_STORE, NoCtx, 32, false>(a, b, d, group_rows, n, rows, lda, ldb, ldd, p, st);
-}
-
-extern "C" int ar_fq_linear_fwd(const ar_qspec* q, const void* x, int64_t t, const void* w, const float* v, const float* mn,
-                                const float* mx, const void* wmin, const void* wmax, const float* gscale, const void* bias,
-                                void* wq_scratch, void* y, void* stream) {
-  AR_REQUIRE(q && x && w && wq_scratch && y && t > 0, AR_E_BADARG, "null pointer");
-  if (int rc = ar_qdq_fwd(q, w, v, mn, mx, wmin, wmax, gscale, wq_scratch, nullptr, nullptr, stream)) return rc;
-  return ar_gemm_bf16(x, wq_scratch, y, (int)t, q->n, q->k, 0, 0, q->k, q->k, q->n, bias, stream);
+  return launch<true, true>(a, b, d, group_rows, n, rows, lda, ldb, ldd, p, st);
 }
 
 extern "C" int ar_fq_linear_bwd_dx(const ar_qspec* q, const void* dy, int64_t t, const void* wq, void* dx, void* stream) {
   AR_REQUIRE(q && dy && wq && dx && t > 0, AR_E_BADARG, "null pointer");
   // dX[T,K] = dY[T,N] · Wq[N,K]:  A = dY (K-major over N), B = Wq viewed as [K_out, N_red] -> MN-major
   return ar_gemm_bf16(dy, wq, dx, (int)t, q->k, q->n, 0, 1, q->n, q->k, q->k, nullptr, stream);
-}
-
-extern "C" int ar_fq_linear_bwd_dw(const ar_qspec* q, const void* dy, const void* x, int64_t t, const void* w, const float* v,
-                                   const float* mn, const float* mx, const void* wmin, const void* wmax, const float* gscale,
-                                   void* dv, int dv_bf16, float* dmin, float* dmax, int accumulate, void* stream) {
-  AR_REQUIRE(q && dy && x && w && dv && t > 0, AR_E_BADARG, "null pointer");
-  if (int rc = check_device()) return rc;
-  const int N = q->n, K = q->k, g = q->group_size;
-  AR_REQUIRE(K % g == 0 && K % 32 == 0, AR_E_UNSUPPORTED, "fused dW epilogue needs K %% group_size == 0 and K %% 32 == 0");
-  const bool is_int = (q->dtype == AR_DT_INT_SYM || q->dtype == AR_DT_INT_ASYM);
-  AR_REQUIRE(!is_int || (wmin && wmax), AR_E_BADARG, "int types need wmin/wmax (ar_group_minmax)");
-  AR_REQUIRE(q->dtype != AR_DT_NV_FP4 || gscale, AR_E_BADARG, "nv_fp4 needs gscale");
-  GemmParams p{};
-  p.dw = DwParams{(const uint16_t*)w, v, mn, mx, (const uint16_t*)wmin, (const uint16_t*)wmax, gscale, dv, dmin, dmax,
-                  q->bits, q->q_scale_thresh, accumulate, dv_bf16, q->init_scale};
-  cudaStream_t st = (cudaStream_t)stream;
-  // D[N_out, K_out] = sum_t dY[t,n] X[t,k]:  A = dY stored [T,N] (MN-major), B = X stored [T,K] (MN-major)
-#define AR_DW(CTX, GG, FP4) \
-  return launch<true, true, EPI_DW, CTX, GG, FP4>(dy, x, nullptr, N, K, (int)t, (int64_t)N, (int64_t)K, 0, p, st)
-  if (q->dtype == AR_DT_INT_SYM) {
-    if (g == 32) AR_DW(IntSym, 32, false);
-    if (g == 64) AR_DW(IntSym, 64, false);
-    if (g == 128) AR_DW(IntSym, 128, false);
-  } else if (q->dtype == AR_DT_INT_ASYM) {
-    if (g == 32) AR_DW(IntAsym, 32, false);
-    if (g == 64) AR_DW(IntAsym, 64, false);
-    if (g == 128) AR_DW(IntAsym, 128, false);
-  } else if (q->dtype == AR_DT_MX_FP4) {
-    if (g == 32) AR_DW(MxFp4, 32, true);
-  } else if (q->dtype == AR_DT_NV_FP4) {
-    if (g == 16) AR_DW(NvFp4, 16, true);
-  }
-#undef AR_DW
-  AR_REQUIRE(false, AR_E_UNSUPPORTED, "fused dW epilogue: dtype %d with group_size %d not built", q->dtype, g);
 }

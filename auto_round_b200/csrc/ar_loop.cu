@@ -1,6 +1,7 @@
-// Per-iteration glue kernels of the sign-SGD loop: masked MSE + gradient, best-iteration bookkeeping,
-// sign-SGD update with best-param snapshot, sample gather.  All HBM-bound, vectorised 16 B accesses,
-// grid = multiple of the SM count, no host synchronisation (state lives in device memory).
+// Per-iteration glue kernels of the sign-SGD loop: masked MSE + gradient, best-iteration bookkeeping, sample gather,
+// device-side schedule (the sign-SGD step itself is part of the per-layer update, ar_fq_update in ar_qdq.cu).  All
+// HBM-bound, vectorised 16 B accesses, grid = multiple of the SM count, no host synchronisation (state lives in device
+// memory).
 #include "ar_common.cuh"
 
 namespace ar {
@@ -72,47 +73,6 @@ __global__ void best_update_kernel(double* loss_sum, double inv_numel, double in
   *loss_sum = 0.0;
 }
 
-__device__ __forceinline__ float sgn(float g) { return (g > 0.f) ? 1.f : ((g < 0.f) ? -1.f : 0.f); }
-
-// g_v: gradient of the rounding segment [0, clamp_begin) (fp32, or bf16 when gv_bf16); g_s: fp32 gradient of the
-// scale segment [clamp_begin, numel), indexed from 0.
-__global__ void __launch_bounds__(256) signsgd_kernel(float* __restrict__ p, const void* __restrict__ g_v, int gv_bf16,
-                                                      const float* __restrict__ g_s, float* __restrict__ best,
-                                                      const int32_t* __restrict__ flag, const float* __restrict__ lr_table,
-                                                      int iter, const int32_t* __restrict__ it_ptr, int64_t n4,
-                                                      int64_t clamp_begin4, float clamp_hi) {
-  if (it_ptr) iter = *it_ptr;
-  const bool snap = (flag != nullptr) && (*flag != 0) && (best != nullptr);
-  const float lr_v = lr_table[2 * iter], lr_s = lr_table[2 * iter + 1];
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 pv = reinterpret_cast<float4*>(p)[i];
-    const bool sc = i >= clamp_begin4;
-    float4 gv;
-    if (sc) {
-      gv = reinterpret_cast<const float4*>(g_s)[i - clamp_begin4];
-    } else if (gv_bf16) {
-      const U2 r = reinterpret_cast<const U2*>(g_v)[i];
-      gv.x = bf16_bits_to_f32((uint16_t)(r.x & 0xffffu)); gv.y = bf16_bits_to_f32((uint16_t)(r.x >> 16));
-      gv.z = bf16_bits_to_f32((uint16_t)(r.y & 0xffffu)); gv.w = bf16_bits_to_f32((uint16_t)(r.y >> 16));
-    } else {
-      gv = reinterpret_cast<const float4*>(g_v)[i];
-    }
-    if (snap) reinterpret_cast<float4*>(best)[i] = pv;
-    const float lr = sc ? lr_s : lr_v;
-    pv.x = pv.x - lr * sgn(gv.x);
-    pv.y = pv.y - lr * sgn(gv.y);
-    pv.z = pv.z - lr * sgn(gv.z);
-    pv.w = pv.w - lr * sgn(gv.w);
-    if (sc) {
-      pv.x = fminf(fmaxf(pv.x, 0.f), clamp_hi);
-      pv.y = fminf(fmaxf(pv.y, 0.f), clamp_hi);
-      pv.z = fminf(fmaxf(pv.z, 0.f), clamp_hi);
-      pv.w = fminf(fmaxf(pv.w, 0.f), clamp_hi);
-    }
-    reinterpret_cast<float4*>(p)[i] = pv;
-  }
-}
-
 __global__ void __launch_bounds__(256) gather_rows_kernel(const U4* __restrict__ src, const int32_t* __restrict__ idx,
                                                           int64_t row_vec, U4* __restrict__ dst) {
   const int64_t s = (int64_t)idx[blockIdx.y] * row_vec, d = (int64_t)blockIdx.y * row_vec;
@@ -160,22 +120,6 @@ extern "C" int ar_best_update(double* loss_sum, double inv_numel, double inv_num
   AR_REQUIRE(loss_sum && state && flag && iter >= 0, AR_E_BADARG, "bad args");
   best_update_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(loss_sum, inv_numel, inv_num_elm, iter, inv_num_elm_ptr, it_ptr, state,
                                                         flag, loss_hist);
-  AR_CHECK_LAUNCH();
-  return AR_OK;
-}
-
-extern "C" int ar_signsgd_step(float* p, const void* g_v, int gv_bf16, const float* g_s, float* best, const int32_t* flag,
-                               const float* lr_table, int iter, const int32_t* it_ptr, int64_t numel, int64_t clamp_begin,
-                               float clamp_hi, void* stream) {
-  AR_REQUIRE(p && g_v && lr_table && iter >= 0 && (g_s || clamp_begin == numel), AR_E_BADARG, "bad args");
-  AR_REQUIRE(numel % 4 == 0 && clamp_begin % 4 == 0, AR_E_UNSUPPORTED, "arena segments must be multiples of 4 floats");
-  const int64_t n4 = numel / 4;
-  int64_t blocks = (n4 + 255) / 256;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  signsgd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(p, g_v, gv_bf16, g_s, best, flag, lr_table, iter, it_ptr,
-                                                                     n4, clamp_begin / 4, clamp_hi);
   AR_CHECK_LAUNCH();
   return AR_OK;
 }

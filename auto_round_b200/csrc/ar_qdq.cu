@@ -326,7 +326,7 @@ struct UpdArgs {
   const int32_t* has_grad; // optional: *has_grad == 0 -> the layer received no gradient this iteration: leave it untouched
 };
 
-// p - lr * sign(g): sign(0) = sign(NaN) = 0 like the kernels of ar_loop.cu
+// p - lr * sign(g), with sign(0) = sign(NaN) = 0
 __device__ __forceinline__ float sign_step(float p, float lr, float g) {
   return (g > 0.f || g < 0.f) ? p - copysignf(lr, g) : p;
 }
@@ -790,27 +790,4 @@ extern "C" int ar_wq_decode(const ar_qspec* q, const void* segments, int64_t seg
       (const uint8_t*)segments, seg_bytes, rows, q->n, q->k, kpad, g, fp4, (uint16_t*)wq_out);
   AR_CHECK_LAUNCH();
   return AR_OK;
-}
-
-// one-to-one aliases of the reference's @register_dtype names
-extern "C" int ar_qdq_int_sym_fwd(const ar_qspec* q, const void* w, const float* v, const float* mn, const float* mx,
-                                  const void* wmin, const void* wmax, void* wq, void* scale, void* stream) {
-  ar_qspec s = *q; s.dtype = AR_DT_INT_SYM;
-  return ar_qdq_fwd(&s, w, v, mn, mx, wmin, wmax, nullptr, wq, scale, nullptr, stream);
-}
-extern "C" int ar_qdq_int_asym_fwd(const ar_qspec* q, const void* w, const float* v, const float* mn,
-                                   const float* mx, const void* wmin, const void* wmax, void* wq, void* scale,
-                                   float* zp, void* stream) {
-  ar_qspec s = *q; s.dtype = AR_DT_INT_ASYM;
-  return ar_qdq_fwd(&s, w, v, mn, mx, wmin, wmax, nullptr, wq, scale, zp, stream);
-}
-extern "C" int ar_qdq_mx_fp4_fwd(const ar_qspec* q, const void* w, const float* v, const float* mx, void* wq,
-                                 void* exp_out, void* stream) {
-  ar_qspec s = *q; s.dtype = AR_DT_MX_FP4;
-  return ar_qdq_fwd(&s, w, v, nullptr, mx, nullptr, nullptr, nullptr, wq, exp_out, nullptr, stream);
-}
-extern "C" int ar_qdq_nv_fp4_fwd(const ar_qspec* q, const void* w, const float* v, const float* mx,
-                                 const float* gscale, void* wq, void* scale, void* stream) {
-  ar_qspec s = *q; s.dtype = AR_DT_NV_FP4;
-  return ar_qdq_fwd(&s, w, v, nullptr, mx, nullptr, nullptr, gscale, wq, scale, nullptr, stream);
 }

@@ -16,8 +16,8 @@ from ._lib import DT_INT_ASYM, DT_INT_SYM, DT_MX_FP4, DT_NV_FP4, QSpec
 # number of kernels of libar_b200.so launched through this module (bench.py reports it as `gpu_launches`)
 LAUNCHES = [0]
 _KERNELS_PER_CALL = {"ar_group_minmax": 1, "ar_absmax": 1, "ar_nv_global_scale": 1, "ar_qdq_fwd": 1, "ar_qdq_bwd": 1,
-                     "ar_gemm_bf16": 1, "ar_fq_linear_fwd": 2, "ar_fq_linear_bwd_dx": 1, "ar_fq_linear_bwd_dw": 1,
-                     "ar_mse_fwd_bwd": 1, "ar_best_update": 1, "ar_sched_load": 1, "ar_iter_advance": 1, "ar_signsgd_step": 1, "ar_gather_rows": 1,
+                     "ar_gemm_bf16": 1, "ar_fq_linear_bwd_dx": 1,
+                     "ar_mse_fwd_bwd": 1, "ar_best_update": 1, "ar_sched_load": 1, "ar_iter_advance": 1, "ar_gather_rows": 1,
                      "ar_pack_int": 3, "ar_unpack_int": 1, "ar_pack_awq": 2, "ar_unpack_awq": 1,
                      "ar_pack_fp4_nv": 1, "ar_pack_fp4_mx": 1, "ar_unpack_fp4": 1}
 
@@ -183,18 +183,6 @@ def gemm(a, b, a_mn_major=False, b_mn_major=False, bias=None, out=None):
     return d
 
 
-def fq_linear_fwd(spec: Spec, x2d, w, v, min_scale, max_scale, wmin, wmax, gscale, bias, wq_scratch, out=None,
-                  init_scale=None):
-    _want(x2d, torch.bfloat16, "x")
-    t = x2d.shape[0]
-    y = out if out is not None else torch.empty(t, spec.n, dtype=torch.bfloat16, device=x2d.device)
-    cs = _cspec(spec, init_scale)
-    _check(_lib.load().ar_fq_linear_fwd(C.byref(cs), _p(x2d), t, _p(w), _p(v), _p(min_scale), _p(max_scale), _p(wmin),
-                                            _p(wmax), _p(gscale), _p(bias), _p(wq_scratch), _p(y), _stream()),
-               "ar_fq_linear_fwd")
-    return y
-
-
 def fq_linear_bwd_dx(spec: Spec, dy2d, wq, out=None):
     _want(dy2d, torch.bfloat16, "dy")
     t = dy2d.shape[0]
@@ -202,19 +190,6 @@ def fq_linear_bwd_dx(spec: Spec, dy2d, wq, out=None):
     cs = spec.c()
     _check(_lib.load().ar_fq_linear_bwd_dx(C.byref(cs), _p(dy2d), t, _p(wq), _p(dx), _stream()), "ar_fq_linear_bwd_dx")
     return dx
-
-
-def fq_linear_bwd_dw(spec: Spec, dy2d, x2d, w, v, min_scale, max_scale, wmin, wmax, gscale, dv, dmin, dmax,
-                     accumulate=False, init_scale=None):
-    _want(dy2d, torch.bfloat16, "dy")
-    _want(x2d, torch.bfloat16, "x")
-    cs = _cspec(spec, init_scale)
-    if dv.dtype not in (torch.float32, torch.bfloat16):
-        raise TypeError("dv must be fp32 or bf16")
-    _check(_lib.load().ar_fq_linear_bwd_dw(C.byref(cs), _p(dy2d), _p(x2d), dy2d.shape[0], _p(w), _p(v), _p(min_scale),
-                                           _p(max_scale), _p(wmin), _p(wmax), _p(gscale), _p(dv),
-                                           int(dv.dtype == torch.bfloat16), _p(dmin), _p(dmax), int(accumulate), _stream()),
-           "ar_fq_linear_bwd_dw")
 
 
 def fq_update(spec: Spec, w, v, min_scale, max_scale, wmin, wmax, gscale, gq, wq_out, lr_table, best_v=None, best_min=None,
@@ -287,21 +262,6 @@ def best_update(loss_sum, inv_numel, inv_num_elm, it, state, flag, loss_hist, in
     """`inv_num_elm_dev` (double [1]) / `it_dev` (int32 [1]) override the host values (CUDA-graph replay)."""
     _check(_lib.load().ar_best_update(_p(loss_sum), float(inv_numel), float(inv_num_elm), int(it), _p(inv_num_elm_dev),
                                       _p(it_dev), _p(state), _p(flag), _p(loss_hist), _stream()), "ar_best_update")
-
-
-def signsgd_step(p, g, best, flag, lr_table, it, clamp_begin, clamp_hi=1.0, it_dev=None, g_scales=None):
-    """`g`: gradient of the rounding segment p[:clamp_begin] (fp32 or bf16) -- or, when `g_scales` is None, one fp32
-    tensor covering the whole arena; `g_scales`: fp32 gradient of p[clamp_begin:]."""
-    _want(p, torch.float32, "p")
-    if g_scales is None:
-        _want(g, torch.float32, "g")
-        g, g_scales = g[:clamp_begin], (g[clamp_begin:] if clamp_begin < p.numel() else None)
-    _want(g_scales, torch.float32, "g_scales")
-    if g.dtype not in (torch.float32, torch.bfloat16):
-        raise TypeError("rounding gradient must be fp32 or bf16")
-    _check(_lib.load().ar_signsgd_step(_p(p), _p(g), int(g.dtype == torch.bfloat16), _p(g_scales), _p(best), _p(flag),
-                                       _p(lr_table), int(it), _p(it_dev), p.numel(), int(clamp_begin), float(clamp_hi),
-                                       _stream()), "ar_signsgd_step")
 
 
 def sched_load(idx_table, inv_num_elm_table, it_dev, count, cur32, cur64, cur_inv):

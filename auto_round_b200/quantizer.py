@@ -70,10 +70,9 @@ def lr_schedule_table(iters: int, lr: float, minmax_lr: float) -> np.ndarray:
 
 class TuneArena:
     """Flat storage for every tunable of one block: fp32 [ V_0 | V_1 | ... | scales ... ] (+ the best snapshot) and the bf16
-    weight gradients `gq` [ dWq_0 | dWq_1 | ... ] written by the grad-w GEMMs.  `with_grads` adds the fp32 pre-sign
-    gradient buffers of the micro-batch path (lm_head: fused grad-w epilogue -> ar_signsgd_step)."""
+    weight gradients `gq` [ dWq_0 | dWq_1 | ... ] written by the grad-w GEMMs."""
 
-    def __init__(self, specs: dict, device, with_grads: bool = False):
+    def __init__(self, specs: dict, device):
         off = 0
         self.views = {}
         for name, spec in specs.items():
@@ -97,20 +96,9 @@ class TuneArena:
             self.gq_views[name] = (goff, spec.n * spec.k, (spec.n, spec.k))
             goff += (spec.n * spec.k + 7) // 8 * 8    # 16-byte aligned segments (TMA store target)
         self.gq = torch.zeros(goff, dtype=torch.bfloat16, device=device)
-        self.grads_v = self.grads_s = None
-        if with_grads:
-            self.grads_v = torch.zeros(self.clamp_begin, dtype=torch.float32, device=device)
-            self.grads_s = torch.zeros(off - self.clamp_begin, dtype=torch.float32, device=device)
 
     def layer_views(self, name: str) -> dict:
-        out = {}
-        for key, (o, n, shape) in self.views[name].items():
-            out[key] = self.params[o:o + n].view(shape)
-            if self.grads_v is not None:
-                if key == "value":
-                    out["grad_" + key] = self.grads_v[o:o + n].view(shape)
-                else:
-                    out["grad_" + key] = self.grads_s[o - self.clamp_begin:o - self.clamp_begin + n].view(shape)
+        out = {key: self.params[o:o + n].view(shape) for key, (o, n, shape) in self.views[name].items()}
         o, n, shape = self.gq_views[name]
         out["gq"] = self.gq[o:o + n].view(shape)
         return out
@@ -187,6 +175,18 @@ class TuneResult:
     batches: list = field(default_factory=list)
     quantized_layers: list = field(default_factory=list)
     used_cuda_graph: bool = False
+
+
+def accumulate_gq(acc: torch.Tensor, gq: torch.Tensor, first: bool, final: bool):
+    """Gradient accumulation over the micro-batches of one iteration: `acc` (fp32) sums the micro-batches' bf16 dWq `gq`
+    (the reference accumulates V.grad in fp32; dV is linear in dWq for fixed parameters), and after the last one the sum
+    is rounded to bf16 once, into `gq`, for the fused update."""
+    if first:
+        acc.copy_(gq)
+    else:
+        acc.add_(gq)
+    if final:
+        gq.copy_(acc)
 
 
 def default_layer_filter(name: str, module: nn.Module) -> bool:
@@ -575,8 +575,6 @@ class SignRoundQuantizer:
         for wl in wrapped.values():
             wl.on_grad = update_layer
 
-        # gradient accumulation: fp32 sums of the micro-batches' bf16 dWq (the reference accumulates V.grad in fp32; dV is
-        # linear in dWq for fixed parameters), rounded to bf16 once for the fused update after the last micro-batch
         acc_state = {"first": True, "final": True}
         gq_acc = {}
         if accum > 1:
@@ -587,13 +585,8 @@ class SignRoundQuantizer:
             gq_acc = {n: torch.zeros(wl.spec.n, wl.spec.k, dtype=torch.float32, device=device) for n, wl in wrapped.items()}
 
             def accumulate_then_update(wl, grad_flag=None):
-                a = gq_acc[name_of[id(wl)]]
-                if acc_state["first"]:
-                    a.copy_(wl.gq)
-                else:
-                    a.add_(wl.gq)
+                accumulate_gq(gq_acc[name_of[id(wl)]], wl.gq, acc_state["first"], acc_state["final"])
                 if acc_state["final"]:
-                    wl.gq.copy_(a)
                     update_layer(wl, grad_flag)
 
             for wl in wrapped.values():
@@ -713,23 +706,25 @@ class SignRoundQuantizer:
     # ---------------------------------------------------------------------------------------------
     def quantize_layer(self, layer: nn.Linear, fp_inputs, q_inputs=None, input_ids=None, name: str = "lm_head", **kwargs):
         """A linear OUTSIDE the block list (lm_head with `quant_lm_head=True`) -- mirror of
-        SignRoundQuantizer.quantize_layer_outside_block (sign_round/quantizer.py:554-759).  Differences from the block loop,
-        all the reference's: micro-batches of one sample with the gradient accumulated over the `batch_size` samples of an
-        iteration (the fused grad-w epilogue runs with accumulate=1), MSELoss(reduction="sum"), the target is the FP weight
-        applied to the FP input (recomputed each step: 128 x [2048, 128256] bf16 targets would be 67 GB for Llama-3), the
-        tuning forward reads the quantised-chain input when there is one, and `num_elm` is fixed before the loop from the
-        first `batch_size` samples.  `fp_inputs` / `q_inputs`: lists of [1, S, K] tensors.  Mutates `layer` in place."""
+        SignRoundQuantizer.quantize_layer_outside_block (sign_round/quantizer.py:554-759), on the block loop's gradient path:
+        bf16 grad-w GEMM, then one fused update (ar_fq_update) per iteration.  Differences from the block loop, all the
+        reference's: micro-batches of one sample with the gradient accumulated over the `batch_size` samples of an
+        iteration (the `accumulate_gq` rule of gradient_accumulate_steps), MSELoss(reduction="sum"), the target is the FP
+        weight applied to the FP input (recomputed each step: 128 x [2048, 128256] bf16 targets would be 67 GB for
+        Llama-3), the tuning forward reads the quantised-chain input when there is one, and `num_elm` is fixed before the
+        loop from the first `batch_size` samples.  `fp_inputs` / `q_inputs`: lists of [1, S, K] tensors.  Mutates `layer`
+        in place."""
         device = layer.weight.device
         if not layer.weight.is_cuda:
             raise RuntimeError("quantize_layer: the layer must be on a CUDA device (no CPU tuning path)")
         torch.cuda.set_device(device)                              # the C ABI launches on the current device's stream
         # Under data parallelism every rank holds the full chained inputs (they were all-gathered) and runs this layer's
         # tuning REPLICATED: identical inputs, identical deterministic kernels, identical result on every rank, no exchange.
-        # (Sharding the micro-batches would need a 2.1 GB fp32 gradient all-reduce per iteration for Llama-3's lm_head.)
+        # (Sharding the micro-batches would need a 1 GB bf16 gradient all-reduce per iteration for Llama-3's lm_head.)
         sc = self.scheme_for(name, layer)
         n, k = layer.weight.shape
         spec = ops.make_spec(sc.qdq_name, sc.bits, sc.group_size, n, k, 1e-5, 1.0)
-        arena = TuneArena({name: spec}, device, with_grads=True)
+        arena = TuneArena({name: spec}, device)
         gs = kwargs.get("nv_global_scale")
         wl = WrapperLinear(layer, sc, spec, arena.layer_views(name), gs)
         nsamples = len(fp_inputs)
@@ -759,28 +754,30 @@ class SignRoundQuantizer:
         flag = torch.zeros(1, dtype=torch.int32, device=device)
         hist = torch.zeros(max(iters, 1), dtype=torch.float32, device=device)
         w, bias = wl.weight, wl.bias_bf16
+        best = arena.best_views(name)
         target = torch.empty(seq, n, dtype=torch.bfloat16, device=device)
         pred = torch.empty_like(target)
         dpred = torch.empty_like(target)
+        gq_acc = torch.empty(n, k, dtype=torch.float32, device=device) if gbs > 1 else None
+        wl.refresh_wq()                                             # iteration 0 runs on qdq(W; V = 0, scales = 1)
         for it in range(iters):
-            for j, i in enumerate(batches[it]):
+            batch = batches[it]
+            for j, i in enumerate(batch):
                 cur = (q_all if q_all is not None else fp_all)[i]
                 ops.gemm(fp_all[i], w, bias=bias, out=target)                                   # layer(org_input), no grad
-                if j == 0:                                          # parameters are fixed inside an iteration: one qdq
-                    ops.fq_linear_fwd(spec, cur, w, wl.value, wl.min_scale, wl.max_scale, wl.weight_min, wl.weight_max,
-                                      wl.weight_global_scale, bias, wl.wq, out=pred)
-                else:
-                    ops.gemm(cur, wl.wq, bias=bias, out=pred)
+                ops.gemm(cur, wl.wq, bias=bias, out=pred)                  # wl.wq is kept current by ar_fq_update
                 ops.mse_fwd_bwd(pred, target, None if token_masks is None else token_masks[i], inv_numel, 1000.0, loss_sum,
                                 dpred=dpred)
-                ops.fq_linear_bwd_dw(spec, dpred, cur, w, wl.value, wl.min_scale, wl.max_scale, wl.weight_min, wl.weight_max,
-                                     wl.weight_global_scale, wl.grad_value, wl.grad_min_scale, wl.grad_max_scale,
-                                     accumulate=(j > 0))
+                ops.gemm(dpred, cur, a_mn_major=True, b_mn_major=True, out=wl.gq)          # dWq = dYᵀ·X, bf16
+                if gq_acc is not None:
+                    accumulate_gq(gq_acc, wl.gq, j == 0, j == len(batch) - 1)
             ops.best_update(loss_sum, inv_numel, 1.0 / float(num_elm), it, state, flag, hist)
             if self.not_use_best_mse:
                 flag.fill_(1 if it == iters - 1 else 0)
-            ops.signsgd_step(arena.params, arena.grads_v, arena.best, flag, lr_tab, it, arena.clamp_begin, 1.0,
-                             g_scales=arena.grads_s)
+            # after the flag: the update snapshots the pre-update parameters when it is set; `it` selects the lr row
+            ops.fq_update(spec, w, wl.value, wl.min_scale, wl.max_scale, wl.weight_min, wl.weight_max, wl.weight_global_scale,
+                          wl.gq, wl.wq, lr_tab, best_v=best["value"], best_min=best.get("min_scale"),
+                          best_max=best["max_scale"], flag=flag, it=it, clamp_hi=1.0)
         if iters > 0:
             self._read_losses(res, state, hist)
             with torch.no_grad():

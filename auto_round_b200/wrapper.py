@@ -8,8 +8,8 @@ hand-written sm_90a kernels behind the C ABI:
     backward  ar_gemm_bf16          dWq = dYᵀ·X  (bf16, like autograd of F.linear)  and  dX = dY · Wq
               ar_fq_update          ONE pass per layer: fake-quant backward from dWq (replaces autograd through
                                     wrapper.py:273-290), best-param snapshot, sign-SGD step, and the NEXT iteration's Wq
-    (layers tuned with micro-batches -- lm_head -- use ar_fq_linear_fwd / ar_fq_linear_bwd_dw, whose GEMM epilogue
-     accumulates the fp32 dV directly)
+    (with micro-batches -- gradient_accumulate_steps, lm_head -- the quantizer sums the micro-batches' dWq in fp32 and
+     runs ar_fq_update once per iteration)
 
 There is no autograd graph over the weight and no eager fallback.
 """
@@ -63,8 +63,8 @@ class _FQLinearFn(torch.autograd.Function):
 
 
 class WrapperLinear(nn.Module):
-    """Wraps an nn.Linear for tuning.  All tensors are CUDA; V / min_scale / max_scale and their gradients are
-    slices of the block arena handed in by the quantizer."""
+    """Wraps an nn.Linear for tuning.  All tensors are CUDA; V / min_scale / max_scale and the bf16 dWq are slices of the
+    block arena handed in by the quantizer."""
 
     def __init__(self, orig_layer: nn.Linear, scheme: QuantizationScheme, spec: ops.Spec, arena_views: dict,
                  global_scale=None, init_scale=None):
@@ -94,10 +94,6 @@ class WrapperLinear(nn.Module):
         self.max_scale = arena_views["max_scale"]
         self.min_scale = arena_views.get("min_scale")
         self.gq = arena_views.get("gq")                     # bf16 [N,K]: dL/dWq of the current iteration
-        # micro-batch layers (quantize_layer): fp32 pre-sign gradients accumulated by the fused grad-w epilogue
-        self.grad_value = arena_views.get("grad_value")
-        self.grad_max_scale = arena_views.get("grad_max_scale")
-        self.grad_min_scale = arena_views.get("grad_min_scale")
         self.on_grad = None                                 # callback(layer) run at the end of this layer's backward
         self.got_grad = False
         self.wq = torch.empty_like(self.weight)            # fake-quant weight of the current iteration

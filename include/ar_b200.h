@@ -62,7 +62,7 @@ typedef struct ar_qspec {
   const float* init_scale; /* NULL, or DEVICE fp32 [N*ceil(K/g)]: enable_alg_ext's searched per-group initial scale
                               (sign_roundv2/quantizer.py:101-125).  int_sym: scale = fp16(init_scale * max_scale), min_scale
                               unused (int.py:201-216); mx/nv: the group amax is multiplied by init_scale * max_scale
-                              (mxfp.py:262-266, nvfp.py:93-97).  Honoured by ar_qdq_fwd/_bwd and ar_fq_linear_*. */
+                              (mxfp.py:262-266, nvfp.py:93-97).  Honoured by ar_qdq_fwd/_bwd and ar_fq_update. */
 } ar_qspec;
 
 /* Per-group min/max of W clamped at 0 (bf16 out, [G]) -- auto_round/wrapper.py:154-167. */
@@ -96,14 +96,6 @@ int ar_qdq_fwd(const ar_qspec* q, const void* w_bf16, const float* v, const floa
 int ar_qdq_bwd(const ar_qspec* q, const void* w_bf16, const float* v, const float* min_scale,
                const float* max_scale, const void* wmin_bf16, const void* wmax_bf16, const float* gscale,
                const float* gq_f32, float* dv, float* dmin, float* dmax, int accumulate, void* stream);
-
-/* named aliases the reference-side registry would bind one-to-one (@register_dtype names) */
-int ar_qdq_int_sym_fwd(const ar_qspec*, const void*, const float*, const float*, const float*, const void*,
-                       const void*, void*, void*, void*);
-int ar_qdq_int_asym_fwd(const ar_qspec*, const void*, const float*, const float*, const float*, const void*,
-                        const void*, void*, void*, float*, void*);
-int ar_qdq_mx_fp4_fwd(const ar_qspec*, const void*, const float*, const float*, void*, void*, void*);
-int ar_qdq_nv_fp4_fwd(const ar_qspec*, const void*, const float*, const float*, const float*, void*, void*, void*);
 
 /*
  * bf16 GEMM on wgmma/TMA:  D[M,N] = A · Bᵀ  with A logical [M,K], B logical [N,K].
@@ -155,30 +147,10 @@ int ar_moe_combine(const void* d_bf16, const void* d2_bf16, const int32_t* row_o
 int ar_moe_rowdot(const void* g_bf16, const void* d_bf16, const int32_t* row_of_pair, int pairs, int topk, int cols,
                   void* dw_bf16, void* stream);
 
-/*
- * Fake-quant linear, forward:  Y[T,N] = X[T,K] · qdq(W)ᵀ (+bias).  wq_scratch (bf16 [N,K]) receives the
- * fake-quant weight once per call (reused by ar_fq_linear_bwd_dx).  = WrapperLinear.forward,
- * auto_round/wrapper.py:517-565.
- */
-int ar_fq_linear_fwd(const ar_qspec* q, const void* x_bf16, int64_t t, const void* w_bf16, const float* v,
-                     const float* min_scale, const float* max_scale, const void* wmin_bf16,
-                     const void* wmax_bf16, const float* gscale, const void* bias_bf16, void* wq_scratch,
-                     void* y_bf16, void* stream);
-/* dX[T,K] = dY[T,N] · Wq[N,K] */
+/* Fake-quant linear, grad-in: dX[T,K] = dY[T,N] · Wq[N,K] (ar_gemm_bf16 with Wq read MN-major).  The forward is
+ * ar_qdq_fwd + ar_gemm_bf16, the weight gradient the grad-w GEMM + ar_fq_update below. */
 int ar_fq_linear_bwd_dx(const ar_qspec* q, const void* dy_bf16, int64_t t, const void* wq_bf16, void* dx_bf16,
                         void* stream);
-/*
- * dWq[N,K] = dYᵀ·X on wgmma with the qdq backward fused in the epilogue: the fp32 accumulator tile goes
- * registers -> shared memory -> (dv, dmin, dmax) without ever materialising dWq.  Outputs are the PRE-sign
- * gradients (sign is taken after the cross-GPU all-reduce, auto_round/.../sign_sgd.py:389).
- * accumulate != 0 adds into dv/dmin/dmax (micro-batches / gradient_accumulate_steps).
- * dv_bf16 != 0: dv is bf16 [N,K] instead of fp32 (only the SIGN of the all-reduced sum is used by the update; bf16
- * halves the per-iteration NVLink exchange of the data-parallel path).
- */
-int ar_fq_linear_bwd_dw(const ar_qspec* q, const void* dy_bf16, const void* x_bf16, int64_t t, const void* w_bf16,
-                        const float* v, const float* min_scale, const float* max_scale, const void* wmin_bf16,
-                        const void* wmax_bf16, const float* gscale, void* dv, int dv_bf16, float* dmin, float* dmax,
-                        int accumulate, void* stream);
 
 /*
  * Fused per-layer update of the sign-SGD loop (one pass, 14 B/weight): given Gq = dL/dWq as bf16 [rows, K] -- the plain
@@ -191,6 +163,8 @@ int ar_fq_linear_bwd_dw(const ar_qspec* q, const void* dy_bf16, const void* x_bf
  *   -> wq_out rows = qdq(W; V', scales') for the next iteration's GEMMs          (WrapperLinear._qdq_weight)
  * v [N,Kpad], min_scale (NULL for mx/nv), max_scale [G] are updated in place; gq is indexed from row gq_row0 (a rank's
  * shard buffer starts at its first row).  dv_dbg/dmn_dbg/dmx_dbg (optional) receive the pre-sign gradients.
+ * lr = lr_table[2*it] for V, lr_table[2*it+1] for the scales, it = *it_ptr when it_ptr is given (CUDA-graph replay),
+ * else iter.
  * has_grad (optional, device): *has_grad == 0 means the layer received no gradient (an expert no token was routed to):
  * SignSGD skips it (sign_sgd.py:274-276), only the best-parameter snapshot still includes it.
  * codes_out / gparams_out (optional, both or none; bits <= 4, not per-row): instead of wq_out the shard's new fake-quant
@@ -229,20 +203,6 @@ int ar_mse_fwd_bwd(const void* pred_bf16, const void* ref_bf16, const uint8_t* r
  */
 int ar_best_update(double* loss_sum, double inv_numel, double inv_num_elm, int iter, const double* inv_num_elm_ptr,
                    const int32_t* it_ptr, double* state, int32_t* flag, float* loss_hist, void* stream);
-
-/*
- * Sign-SGD step over a flat fp32 arena [ V of all layers | min/max_scale of all layers ]
- * (SignSGD.step, sign_sgd.py:356-389, + the [0,hi] clamp the next forward would apply to min/max_scale,
- * wrapper.py:257-259):
- *   if (*flag) best[i] = p[i];           (collect_best_params, compressors/utils.py:205-217: PRE-update values)
- *   p[i] -= lr * sign(g[i]);  for i >= clamp_begin: p[i] = clamp(p[i], 0, clamp_hi)
- *   g_round covers [0, clamp_begin) (fp32, or bf16 if g_round_bf16); g_scales (fp32) covers [clamp_begin, numel).
- * lr_table[2*iter] (rounding lr) / lr_table[2*iter+1] (minmax lr) are read on the device so the step can live in
- * a CUDA graph.  numel and clamp_begin must be multiples of 4.
- */
-int ar_signsgd_step(float* p, const void* g_round, int g_round_bf16, const float* g_scales, float* best,
-                    const int32_t* flag, const float* lr_table, int iter, const int32_t* it_ptr, int64_t numel,
-                    int64_t clamp_begin, float clamp_hi, void* stream);
 
 /*
  * Device-side loop schedule (replaces the python loop variable so that one iteration = one CUDA graph):

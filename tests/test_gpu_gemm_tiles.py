@@ -1,10 +1,12 @@
 """GPU checks of what the 128 x 256 store tiles and the register-to-global epilogue of ar::gemm_kernel can break: ragged
 edges in n (not a multiple of the 256-wide tile), m and k, bias, column-slice outputs with a row pitch wider than n,
-run-to-run determinism under the dynamic tile scheduler, and the grouped MoE launches with ragged n.
+run-to-run determinism under the dynamic tile scheduler, a launch from a thread without a current CUDA context, and the
+grouped MoE launches with ragged n.
 
 Tolerance (same as the GEMM checks of test_gpu_kernels.py): fp32-accumulated bf16 products against an fp32 torch
 reference, |d - ref| <= 2^-7*|ref| + 2e-3*rms(ref)."""
 import ctypes as C
+import threading
 
 import pytest
 import torch
@@ -83,6 +85,28 @@ def test_repeat_launch_bit_identical(a_mn, b_mn):
     assert torch.equal(d1, d2)
     rows = torch.randint(0, m, (64,), device=DEV)
     _close(d1[rows], _ref(a, b, a_mn, b_mn)[rows])
+
+
+def test_launch_from_a_thread_without_a_context():
+    """The first GEMM of a thread that has made no CUDA runtime call, as PyTorch's autograd device threads start: encoding
+    the TMA descriptors needs a current context, and the launch makes the device's primary context current itself."""
+    a, b = _operands(256, 512, 128, False, False, seed=4)
+    want = ops.gemm(a, b)
+    got = torch.empty_like(want)
+    err = []
+
+    def run():
+        try:
+            ops.gemm(a, b, out=got)
+        except Exception as e:  # noqa: BLE001 -- reported by the assertion below
+            err.append(e)
+
+    t = threading.Thread(target=run)
+    t.start()
+    t.join()
+    assert not err, err[0]
+    torch.cuda.synchronize()
+    assert torch.equal(got, want)
 
 
 def _route(tokens, e, topk, skip):

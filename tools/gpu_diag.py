@@ -72,14 +72,9 @@ for (n, k, tag) in [(4096, 4096, "q_proj"), (14336, 4096, "gate_proj"), (4096, 1
         mn = torch.ones(spec.groups, device=dev)
         mx = torch.ones(spec.groups, device=dev)
         wmin, wmax = ops.group_minmax(spec, w)
-        dv = torch.empty(n, k, device=dev)
-        dmin = torch.empty(spec.groups, device=dev)
-        dmax = torch.empty(spec.groups, device=dev)
-        t_dwf = timeit(lambda: ops.fq_linear_bwd_dw(spec, dy, x, w, v, mn, mx, wmin, wmax, None, dv, dmin, dmax))
         wq = torch.empty_like(w)
         t_qdq = timeit(lambda: ops.qdq_fwd(spec, w, v, mn, mx, wmin, wmax, None, out_wq=wq))
-        rec.update(dw_fused_ms=t_dwf, dw_fused_tflops=fl / t_dwf / 1e9, qdq_ms=t_qdq,
-                   qdq_gbs=(n * k * 8) / t_qdq / 1e6)
+        rec.update(qdq_ms=t_qdq, qdq_gbs=(n * k * 8) / t_qdq / 1e6)
     except Exception as e:  # noqa: BLE001
         rec = {"layer": tag, "error": repr(e)}
     out["timing"].append(rec)

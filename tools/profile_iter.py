@@ -37,7 +37,7 @@ with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
     torch.cuda.synchronize()
 ev = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
 ev.sort(key=lambda e: e.time_range.start)
-# isolate steady-state iterations: between consecutive signsgd kernels
+# isolate steady-state iterations: between consecutive iter_advance kernels
 idx = [i for i, e in enumerate(ev) if "iter_advance" in e.name]
 lines = []
 if len(idx) >= 8:
