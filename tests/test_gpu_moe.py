@@ -41,7 +41,11 @@ def _routing(tokens, e, k, seed, skip_expert=None):
     return idx, (w / w.sum(-1, keepdim=True)).bfloat16()
 
 
-@pytest.mark.parametrize("tokens,e,k,e_begin,e_local", [(300, 4, 2, 0, 4), (1000, 8, 2, 0, 8), (1000, 8, 2, 4, 4), (257, 3, 1, 1, 2)])
+@pytest.mark.parametrize("tokens,e,k,e_begin,e_local", [(300, 4, 2, 0, 4), (1000, 8, 2, 0, 8), (1000, 8, 2, 4, 4), (257, 3, 1, 1, 2),
+                                                        (16384, 8, 2, 0, 8),       # Mixtral at a production token count
+                                                        (4096, 128, 8, 64, 32),    # EP rank at the 32-local-expert limit
+                                                        (2048, 64, 8, 32, 32),
+                                                        (5, 32, 1, 0, 32)])        # fewer pairs than threads
 def test_route_tables(tokens, e, k, e_begin, e_local):
     idx, _ = _routing(tokens, e, k, seed=tokens)
     ids = idx.reshape(-1).to(DEV)
