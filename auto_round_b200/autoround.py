@@ -14,6 +14,7 @@ AutoScheme, MLLM / diffusion calibration, torch.compile, CPU execution.
 from __future__ import annotations
 
 import json
+import logging
 import os
 import random
 import time
@@ -30,6 +31,8 @@ from .moe import unfuse_experts
 from .quantizer import DataParallel, SignRoundQuantizer, valid_token_masks
 from .schemes import QuantizationScheme, parse_scheme
 from .wrapper import set_module
+
+logger = logging.getLogger(__name__)
 
 _SCHEME_KW = ("bits", "group_size", "sym", "data_type", "act_bits", "act_group_size", "act_sym", "act_data_type",
               "act_dynamic", "super_bits", "super_group_size")
@@ -59,6 +62,34 @@ def find_blocks(model: nn.Module):
             if any(isinstance(sub, nn.Linear) for sub in mod[0].modules()):
                 return name, mod
     raise RuntimeError("no transformer block list found in the model")
+
+
+def block_groups(nblk: int, nblocks: int) -> list:
+    """Indices of the blocks tuned together: [i, min(i + nblocks, nblk)) for i = 0, nblocks, 2 nblocks, ...; the last
+    group may be short (compressors/orchestrator.py:227-241)."""
+    return [list(range(i, min(i + nblocks, nblk))) for i in range(0, nblk, nblocks)]
+
+
+class BlockGroup(nn.Module):
+    """Consecutive decoder blocks tuned as one unit (nblocks > 1): the forward feeds each member's first output to the
+    next member, every member with the same kwargs, and returns the last member's output.  The members stay where they are
+    in the model; the group only holds them, as `layers.<j>`."""
+
+    def __init__(self, blocks, names):
+        super().__init__()
+        self.layers = nn.ModuleList(blocks)
+        self.names = list(names)
+
+    def prefix_map(self) -> dict:
+        """{"layers.<j>": full name of member j}: the group-relative name of a layer -> its full module name
+        (SignRoundQuantizer.layer_names)."""
+        return {f"layers.{j}": n for j, n in enumerate(self.names)}
+
+    def forward(self, hidden_states, *args, **kwargs):
+        for blk in self.layers:
+            out = blk(hidden_states, *args, **kwargs)
+            hidden_states = out[0] if isinstance(out, (tuple, list)) else out
+        return hidden_states
 
 
 def repeated_tail(input_ids: torch.Tensor) -> torch.Tensor:
@@ -210,8 +241,14 @@ class AutoRound:
         self.quant_lm_head = bool(kwargs.get("quant_lm_head"))
         if kwargs.get("dynamic_max_gap", -1) not in (-1, None) or kwargs.get("momentum") not in (None, 0, 0.0):
             raise NotImplementedError("dynamic_max_gap / momentum: only the reference defaults (-1 / 0)")
-        if kwargs.get("nblocks", 1) != 1:
-            raise NotImplementedError("nblocks != 1")
+        nblocks = kwargs.get("nblocks", 1)
+        if nblocks is None:
+            nblocks = 1
+        if isinstance(nblocks, bool) or not isinstance(nblocks, int) or nblocks <= 0:
+            raise ValueError(f"`nblocks` must be a positive int, got {nblocks!r}")
+        # nblocks > 1: SignRound tunes each run of `nblocks` consecutive blocks as one BlockGroup (one loss at the group's
+        # output, one arena, one best iteration); the RTN modes (iters == 0) ignore it
+        self.nblocks = nblocks
         self.model = model.eval()
         self.tokenizer = tokenizer
         self.scheme: QuantizationScheme = parse_scheme(scheme, {k: kwargs.get(k) for k in _SCHEME_KW})
@@ -496,13 +533,19 @@ class AutoRound:
         # above 8 bits still joins the shared NVFP4 global scale of its q/k/v or gate/up group; the calibrated modes
         # list only the layers they quantize.
         all_linears = mode in ("plain", "zero_shot_opt")
-        for bi, block in enumerate(blocks):
+        for group in block_groups(nblk, self.nblocks if tune else 1):
+            bi = group[0]
             if bi < start:
                 continue
             tb = time.time()
-            quantizer.block_prefix = f"{prefix}.{bi}"                     # layer_config keys are full module names
+            if self.nblocks == 1 or not tune:
+                block = blocks[bi]
+                quantizer.block_prefix = f"{prefix}.{bi}"                 # layer_config keys are full module names
+            else:                                                         # the group is tuned as one module
+                block = BlockGroup([blocks[j] for j in group], [f"{prefix}.{j}" for j in group])
+                quantizer.block_prefix = block.prefix_map()
             self._hook(bi, "h2d0")
-            block.to(self.device)                                         # H2D of this block's weights
+            block.to(self.device)                                         # H2D of this block's (group's) weights
             unfuse_experts(block)                                         # MoE: fused 3-D experts -> per-expert nn.Linear
             self._freeze(block)
             self._hook(bi, "compute0")
@@ -529,7 +572,7 @@ class AutoRound:
                 done = res.quantized_layers
                 ev[2].record()
                 # (6) outputs of the quantised block feed the next block (composer.py:476-481)
-                if quantizer.enable_quanted_input and (bi + 1 < nblk or self.quant_lm_head):
+                if quantizer.enable_quanted_input and (group[-1] + 1 < nblk or self.quant_lm_head):
                     q_inputs = self._forward_all(quantizer, block, eff, others, token_masks)
                 else:
                     q_inputs = None
@@ -566,10 +609,12 @@ class AutoRound:
                     resume.mark_block_done(f"{prefix}.{bi}", snap, q_inputs, fp_inputs)
                 phases = {k: ev[i].elapsed_time(ev[i + 1])
                           for i, k in enumerate(("ref_forward_ms", "tune_ms", "q_forward_ms", "pack_ms"))}
-                self.block_results.append({"block": f"{prefix}.{bi}", "init_loss": res.init_loss, "best_loss": res.best_loss,
-                                           "best_iter": res.best_iter, "seconds": time.time() - tb, "losses": res.losses,
-                                           "phases_ms": phases, "cuda_graph": res.used_cuda_graph, "batches": res.batches,
-                                           "block_mse": blk_mse})
+                rec = {"block": f"{prefix}.{bi}", "init_loss": res.init_loss, "best_loss": res.best_loss,
+                       "best_iter": res.best_iter, "seconds": time.time() - tb, "losses": res.losses,
+                       "phases_ms": phases, "cuda_graph": res.used_cuda_graph, "batches": res.batches, "block_mse": blk_mse}
+                if isinstance(block, BlockGroup):
+                    rec["blocks"] = list(block.names)
+                self.block_results.append(rec)
             elif mode == "calibrated_opt":
                 rec = {"block": f"{prefix}.{bi}", "imatrix_layers": len(imatrices)}
                 if getattr(self, "keep_imatrix", False):                  # inspection hook for the parity tests
@@ -659,6 +704,10 @@ class AutoRound:
         """-> (ResumeState | None, index of the first block still to do).  Active only when AR_RESUME_DIR is set."""
         rd = os.environ.get("AR_RESUME_DIR")
         if not rd:
+            return None, 0
+        if self.nblocks != 1:              # orchestrator.py:226, :696-701: no resume inside or across groups
+            logger.warning("AR_RESUME_DIR is set but nblocks=%d: resume state is kept only for nblocks=1, so this run "
+                           "starts from block 0 and writes none", self.nblocks)
             return None, 0
         names = [f"{prefix}.{i}" for i in range(len(blocks))]
         model_id = getattr(getattr(self.model, "config", None), "_name_or_path", None)

@@ -146,8 +146,14 @@ class fused_block_ops:
                     and "forward" not in m.__dict__:
                 m.forward = types.MethodType(_fused_mlp_forward, m)
                 self.mlps.append(m)
-        mod = sys.modules.get(type(self.block).__module__)
-        fn = getattr(mod, "apply_rotary_pos_emb", None) if mod is not None else None
+        # the rotary helper of the model file that defines the block: for a group of blocks tuned together (nblocks > 1)
+        # that is the file of its members, the first modules of the walk that have one
+        fn = None
+        for m in self.block.modules():
+            mod = sys.modules.get(type(m).__module__)
+            fn = getattr(mod, "apply_rotary_pos_emb", None) if mod is not None else None
+            if fn is not None:
+                break
         if fn is not None and not getattr(fn, "_ar_fused", False):
             self.rope = (mod, fn)
             mod.apply_rotary_pos_emb = _make_fused_rope(fn)

@@ -303,16 +303,30 @@ class SignRoundQuantizer:
         if self.not_use_best_mse:
             res.best_iter, res.best_loss = self.iters - 1, res.losses[-1]
 
+    def layer_names(self, name: str):
+        """(full module name or None, name inside its own decoder block) of a layer named `name` relative to the module being
+        tuned.  `self.block_prefix`, set by AutoRound before each block, is the block's full name ("model.layers.3"), or
+        for a group of blocks tuned together (nblocks > 1) the prefix map of its `BlockGroup` ({"layers.0":
+        "model.layers.2", "layers.1": "model.layers.3"}), which sends "layers.1.mlp.down_proj" to
+        ("model.layers.3.mlp.down_proj", "mlp.down_proj")."""
+        prefix = getattr(self, "block_prefix", None)
+        if not prefix:
+            return None, name
+        if isinstance(prefix, str):
+            return f"{prefix}.{name}", name
+        head, j, rel = name.split(".", 2)
+        return f"{prefix[f'{head}.{j}']}.{rel}", rel
+
     def scheme_for(self, name: str, module: nn.Module) -> Optional[QuantizationScheme]:
         """Per-layer override: `layer_config` keys are FULL module names as in the reference
-        ("model.layers.3.mlp.down_proj": {"bits": 8}); `self.block_prefix` ("model.layers.3", set by AutoRound before each
-        block) turns the block-relative `name` into one.  A bare block-relative key applies to that layer of every block."""
+        ("model.layers.3.mlp.down_proj": {"bits": 8}); `layer_names` turns the block-relative `name` into one.  A bare
+        block-relative key ("mlp.down_proj") applies to that layer of every block."""
         cfg = None
-        prefix = getattr(self, "block_prefix", None)
-        if prefix:
-            cfg = self.layer_config.get(f"{prefix}.{name}")
+        full, rel = self.layer_names(name)
+        if full:
+            cfg = self.layer_config.get(full)
         if cfg is None:
-            cfg = self.layer_config.get(name)
+            cfg = self.layer_config.get(rel)
         if cfg is None:
             return self.scheme
         if isinstance(cfg, QuantizationScheme):
